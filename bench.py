@@ -2,14 +2,16 @@
 """bench.py -- dispatch LPs/sec on BASELINE.json's headline config (C2: wind+battery, 24 periods, 10 000
 synthetic LMP scenarios per GPU), one JSON line on rank 0.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
   torchrun --nproc-per-node N bench.py --gpus N ...        (one rank per GPU, weak scaling: 10 000 LPs per rank,
                                                             one all_gather of the objectives per step)
 
 A "step" = one pass of the hot path over one batch: parameter rows already in HBM -> one kernel launch ->
 obj/status/iters in HBM (`value`), or through the host C-ABI call with H2D / D2H inside the timed region (`e2e`).
 `--impl reference` times the CPU path the reference would take for these LPs (restated LP + HiGHS in a process
-pool over all host cores; CBC/IPOPT/Pyomo are not installable here, see DESIGN.md).
+pool over all host cores; CBC/IPOPT/Pyomo are not dependencies of this project, see DESIGN.md).
+`--dump-outputs DIR` writes what the last timed step returned (obj, status, iters of rank r's batch) as float64 .npy files,
+so that two builds can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -32,7 +34,8 @@ BATCH = 10000
 METRIC = "dispatch LPs/sec (24-period price-taker batch); max |obj| rel-err vs IPOPT"
 ALG_BYTES_PER_LP = 8 * T + 8 + 4 + 4           # lmp row in; obj, status, iters out (SURVEY.md §8d: 208 B)
 ALG_FLOP_PER_LP = 0.30e6                       # banded-IPM algorithmic FP64 flops per LP (SURVEY.md §8d)
-FP64_PEAK_TFLOPS_NOMINAL = 37.0                # HGX B200 spec sheet (296 TF / 8 GPUs); no measured FP64 peak file
+FP64_PEAK_TFLOPS_NOMINAL = 34.0                # H100 SXM data sheet, FP64 without tensor cores (700 W card)
+HBM_PEAK_GBS_NOMINAL = 3350.0                  # H100 SXM data sheet, HBM3
 
 
 def workload(rank):
@@ -243,6 +246,7 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the C3/C4/C5 block")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":
@@ -317,6 +321,10 @@ def main():
     t_wall = time.perf_counter() - t_wall0
     launches = S.launch_count() - n0
     out = outs[(args.steps - 1) % len(outs)]
+    if args.dump_outputs:
+        # copied before anything else reuses the buffers: the sustained loop below writes into `out` again
+        suffix = f"_rank{rank}" if world > 1 else ""
+        dump = {name + suffix: getattr(out, name).cpu().numpy().astype(np.float64) for name in ("obj", "status", "iters")}
     step_ms = sum(a.elapsed_time(b) for a, b, _ in ev) + ev_tail[0].elapsed_time(ev_tail[1])
     kern_ms = sum(a.elapsed_time(c) for a, _, c in ev)
     tt = torch.tensor([step_ms, kern_ms], dtype=torch.float64, device=dev)
@@ -374,28 +382,21 @@ def main():
     if world > 1:                              # all collectives are done: every rank leaves the group together
         torch.cuda.synchronize()
         dist.destroy_process_group()
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), a)
     if rank != 0:
         return
     total = BATCH * world
     value = total * args.steps / (step_ms * 1e-3)
-    peaks = {}
-    pk = ROOT / "MEASURED_PEAKS.json"
-    if pk.exists():
-        peaks = json.load(open(pk))
-    hbm_peak, which = (peaks.get("hbm_gbs"), "measured (MEASURED_PEAKS.json)") if peaks.get("hbm_gbs") else (6650.0, "fallback")
+    hbm_peak, which = HBM_PEAK_GBS_NOMINAL, "nominal (H100 SXM data sheet)"
     kern_s = kern_ms * 1e-3 / args.steps
     ach = ALG_BYTES_PER_LP * BATCH / kern_s / 1e9
     fp64 = ALG_FLOP_PER_LP * BATCH / kern_s / 1e12
     fp64_peak = S.fp64_peak_tflops()
     if not fp64_peak > 0:
         fp64_peak = None
-    # DRAM bytes per launch of the dominant kernel from the committed ncu capture (profiles/), not measured live
-    traffic = None
-    try:
-        cur = json.load(open(ROOT / "profiles" / "current.json"))["stage_profile"]
-        traffic = float(json.load(open(ROOT / "profiles" / cur))["traffic_bytes_per_launch"])
-    except Exception:
-        pass
     line = {"metric": METRIC, "value": value, "unit": "LPs/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": step_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f64", "data": "synthetic", "config": config(world),
@@ -404,10 +405,10 @@ def main():
                     "api": "dsp_lp_solve_batch_host (C-ABI, host buffers)"},
             "gpu_launches": int(launches), "kernel_ms_per_step": kern_ms / args.steps,
             "roofline": {"bound": "fp64", "achieved": fp64, "peak": fp64_peak or FP64_PEAK_TFLOPS_NOMINAL, "unit": "TFLOP/s",
-                         "frac": fp64 / (fp64_peak or FP64_PEAK_TFLOPS_NOMINAL), "traffic": traffic,
+                         "frac": fp64 / (fp64_peak or FP64_PEAK_TFLOPS_NOMINAL),
                          "alg_flop_per_lp": ALG_FLOP_PER_LP, "alg_bytes_per_launch": ALG_BYTES_PER_LP * BATCH,
-                         "peak_source": "measured DFMA micro-benchmark on this GPU (dsp_lp_fp64_peak_tflops); MEASURED_PEAKS.json has no FP64 entry"
-                                        if fp64_peak else "nominal (HGX B200 spec 296 TF / 8)",
+                         "peak_source": "measured DFMA micro-benchmark on this GPU (dsp_lp_fp64_peak_tflops)"
+                                        if fp64_peak else "nominal (H100 SXM data sheet)",
                          "peak_tflops_nominal": FP64_PEAK_TFLOPS_NOMINAL,
                          "note": "on-chip FP64 solve: bound by FP64 issue + dependent-chain latency, not HBM or tensor cores (SURVEY.md 8d); "
                                  "achieved = algorithmic banded-IPM flops (0.30 MFLOP/LP) / kernel time",

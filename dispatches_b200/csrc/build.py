@@ -1,8 +1,8 @@
-"""Builds libdsp_lp.so (the C-ABI of include/dsp_lp.h) in-tree for sm_100a with nvcc.
+"""Builds libdsp_lp.so (the C-ABI of include/dsp_lp.h) in-tree for sm_90a (H100) with nvcc.
 
     python -m dispatches_b200.csrc.build [--force]
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels to the GPU box with the snapshot.
+nvcc cross-compiles without a GPU.  The .so is a build product and is git-ignored.
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
 LIB = HERE / "libdsp_lp.so"
 SOURCES = [HERE / "dsp_lp.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", f"-I{ROOT / 'include'}"]
 
 
@@ -37,7 +37,10 @@ def needs_build():
 
 def build(force=False, verbose=False):
     """Builds the library if sources are newer.  Serialised across processes with a file lock: under torchrun every rank
-    calls this at start-up and only the first one may run nvcc."""
+    calls this at start-up and only the first one may run nvcc.  An up-to-date library is returned without touching the
+    tree, so that a built checkout can be used read-only."""
+    if not force and not needs_build():
+        return LIB
     import fcntl
     with open(HERE / ".build.lock", "w") as lk:
         fcntl.flock(lk, fcntl.LOCK_EX)

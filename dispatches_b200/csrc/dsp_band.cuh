@@ -8,9 +8,8 @@
 // The sweeps walk the band IN PLACE: every pivot step is load -> FMA -> store -> __syncwarp on the memory the band lives in -- shared
 // memory in the "smem" / "hybrid" placements of dsp_lp.cu, the L1-cached global workspace in the "ws" placement (the active window of
 // a sweep stays in L1, so a step costs about the same there).  A register-window variant (active window in registers sliding by warp
-// shuffles, band streamed with loads issued 8 steps ahead; bit-identical results on the emulator) was measured on the B200 and
-// REJECTED: C4 50.0 vs 39.1 ms, wind+PEM T = 2184 494 vs 458 ms (profiles/band_rw_r2.log) -- in the workspace placement the time is in the
-// element-wise / CSR passes that stream the per-LP vectors through L2, not in the sweeps.
+// shuffles, band streamed with loads issued 8 steps ahead; bit-identical results on the emulator) was tried and rejected as
+// slower -- in the workspace placement the time is in the element-wise / CSR passes that stream the per-LP vectors through L2, not in the sweeps.
 //
 // Plain C++ over warp builtins: tests/emu compiles this file with g++ on the SIMT emulator and checks it against a dense solve.
 #pragma once

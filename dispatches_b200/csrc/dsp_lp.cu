@@ -1,4 +1,4 @@
-// dsp_lp.cu -- batched primal-dual interior-point LP solver for sm_100a (B200).  C ABI: include/dsp_lp.h
+// dsp_lp.cu -- batched primal-dual interior-point LP solver for sm_90a (H100).  C ABI: include/dsp_lp.h
 //
 // Replaces the per-scenario  SolverFactory("cbc").solve(m)  loop of the reference's price-taker sweeps
 // (wind_battery_LMP.py:266-267, wind_battery_PEM_LMP.py:296-298, price_taker_analysis.py:365-403) by one
@@ -30,7 +30,7 @@
 
 #include "dsp_band.cuh"
 
-#define DSP_VERSION "dsp_lp 0.2 (sm_100a band-IPM + stage kernels)"
+#define DSP_VERSION "dsp_lp 0.2 (sm_90a band-IPM + stage kernels)"
 
 namespace {
 
@@ -546,12 +546,12 @@ namespace {
 #ifndef DSP_S2_WARPS
 #define DSP_S2_WARPS 8
 #endif
-constexpr int kStage2Warps = DSP_S2_WARPS;        // warps per CTA = per SM: 8 x 27.9 KB of shared memory, 8 x 32 x 255 registers.  (9 warps would
-                                                 // make a 10 000-LP batch two waves instead of three, but the register file is per scheduler:
-                                                 // a third warp on one of the four caps every thread at 168 registers -- 2 KB of spills)
+constexpr int kStage2Warps = DSP_S2_WARPS;        // warps per CTA = per SM: 8 x 27.9 KB of shared memory, 8 x 32 x 255 registers.  (A ninth
+                                                 // warp does not fit the register file, which is per scheduler: a third warp on one of the
+                                                 // four caps every thread at 168 registers -- 2 KB of spills)
 // warps per CTA (= per SM) of the chain kernel: what shared memory allows at 168 registers per thread (three warps on a scheduler).
-// NF = 2 (19.5 KB per warp): 11 warps -- 3 256 group slots at L = 16, so the 5 000 LPs of C3 are two waves instead of the three
-// they were at 8 warps / 219 registers (0.42 -> see profiles/chain1_warps_r2.log); NF = 3 (24.8 KB per warp): 8
+// NF = 2 (19.5 KB per warp): 11 warps -- 2 904 group slots at L = 16 on the 132 SMs of an H100, so the 5 000 LPs of C3 are two
+// waves instead of the three they are at 8 warps / 219 registers; NF = 3 (24.8 KB per warp): 8
 constexpr int chain1_warps(int NF) { return NF == 2 ? 11 : 8; }
 template <int L, int P, bool SYNC>
 __global__ void __launch_bounds__(32 * kStage2Warps, 1) dsp_ipm_stage2_wb_kernel(const stage2::Params Q) {
@@ -595,8 +595,8 @@ inline Stage2Geom stage2_geometry(int T) {
 }
 constexpr int kStage2MaxT = 96;
 
-// FP64 FMA micro-benchmark: the measured denominator of the FP64 roofline fraction bench.py reports (the driver's
-// MEASURED_PEAKS.json has HBM and bf16 peaks only).  8 independent DFMA chains per thread.
+// FP64 FMA micro-benchmark: the measured denominator of the FP64 roofline fraction bench.py reports.  8 independent DFMA
+// chains per thread.
 __global__ void __launch_bounds__(256) dsp_fp64_peak_kernel(double *out, int iters, double a, double b) {
     double x0 = threadIdx.x, x1 = x0 + 1, x2 = x0 + 2, x3 = x0 + 3, x4 = x0 + 4, x5 = x0 + 5, x6 = x0 + 6, x7 = x0 + 7;
     for (int i = 0; i < iters; ++i) {
@@ -653,6 +653,7 @@ struct dsp_template {
     int device;
     int sm_count;
     int smem_optin;
+    size_t ws_cap;                 // largest global workspace a launch may allocate: a quarter of device memory
     std::vector<void *> dev_allocs;
     std::vector<int> col_perm, row_perm;     // dsp_lp_template_create_csr: caller index of internal column / row
     std::vector<int> csr_ptr, csr_idx, asm_qa, asm_qb;   // permuted CSR pattern + assembly factor positions (kept for matrix parameters)
@@ -827,6 +828,7 @@ int dsp_lp_template_create(const dsp_template_desc *D, dsp_template **out) {
     CK(cudaGetDeviceProperties(&prop, T->device));
     T->sm_count = prop.multiProcessorCount;
     T->smem_optin = (int)prop.sharedMemPerBlockOptin;
+    T->ws_cap = prop.totalGlobalMem / 4;
     KParams &K = T->kp;
     K.m = m; K.n = n; K.nb = nb; K.w = wt; K.Pc = D->Pc; K.Pr = D->Pr; K.nnz = nnz; K.nasm = nasm;
     K.hot_bytes = (int)hot_bytes;
@@ -987,12 +989,12 @@ void dsp_lp_template_destroy(dsp_template *T) {
 }
 
 // Geometry of a band-kernel launch: one persistent CTA per SM, `warps` LPs in flight per CTA, and one of three
-// placements of the per-LP work region (measured on the B200: profiles/band_modes_r1.json, ws_mode_sweep*_r1.json):
+// placements of the per-LP work region:
 //   smem    everything in shared memory: fastest warp, but only as many LPs per SM as regions fit;
 //   hybrid  the (dy, Mb) tail -- all that the LDL' / substitution sweeps touch -- in shared memory, the element-wise
-//           vectors in a global workspace (coalesced streaming through L2): a warp runs at ~0.3-0.45 of the smem speed;
-//   ws      everything in the global workspace, kMaxWarps LPs per SM: a warp runs at ~1/6 of the smem speed (L2 latency
-//           in the sweeps); the only choice for long horizons (T = 8736).
+//           vectors in a global workspace (coalesced streaming through L2): a slower warp, but more LPs per SM;
+//   ws      everything in the global workspace, kMaxWarps LPs per SM: slower still per warp (L2 latency in the sweeps);
+//           the only choice for long horizons (T = 8736).
 struct BandGeom { long long warps; int hot_in_smem; size_t off; bool ws; int hybrid; };
 
 BandGeom band_geometry(const dsp_template *T, const KParams &K) {
@@ -1030,7 +1032,7 @@ BandGeom band_geometry(const dsp_template *T, const KParams &K) {
         if (g.hybrid && hybrid2) g.hybrid = 2;
 #endif
         g.warps = g.hybrid ? hybrid_warps : kMaxWarps;
-        while (g.warps > 1 && (size_t)T->sm_count * (size_t)g.warps * prob_bytes > ((size_t)48 << 30)) g.warps /= 2;
+        while (g.warps > 1 && (size_t)T->sm_count * (size_t)g.warps * prob_bytes > T->ws_cap) g.warps /= 2;
     }
     g.warps = std::min<long long>(g.warps, kMaxWarps);
     return g;
@@ -1061,7 +1063,7 @@ static int launch_batch(const dsp_template *T, int64_t N, const double *cparams,
         int occ = 0;
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dsp_ipm_stage2_long_kernel, 32 * kLongWarps, 0));
         long long warps = std::min<long long>(N, (long long)T->sm_count * std::max(occ, 1) * kLongWarps);
-        while (warps > 1 && (size_t)warps * per_warp > ((size_t)64 << 30)) warps /= 2;
+        while (warps > 1 && (size_t)warps * per_warp > T->ws_cap) warps /= 2;
         // spread the warps over the SMs: one warp per CTA while there are fewer LPs than SMs x kLongWarps
         const int wpb = (int)std::min<long long>(kLongWarps, std::max<long long>(1, warps / T->sm_count));
         const long long blocks = (warps + wpb - 1) / wpb;
@@ -1093,8 +1095,8 @@ static int launch_batch(const dsp_template *T, int64_t N, const double *cparams,
             g_last_grid = (int)blocks; g_last_block = 32 * wpb; g_last_smem = 0; g_last_ppc = wpb;
         }
         // At T = 8736 cond(M) reaches 1e15 and the partitioned elimination order rounds differently from the band kernel's
-        // sequential one: about 1 LP in 60 of the reference's full-year sweep stalls here and converges there
-        // (profiles/long_hard_r2.log).  The band kernel therefore follows on the same stream and re-solves ONLY the LPs this
+        // sequential one: about 1 LP in 60 of the reference's full-year sweep stalls here and converges there.
+        // The band kernel therefore follows on the same stream and re-solves ONLY the LPs this
         // kernel left with MAX_ITER / NUMERICAL (its warps skip every other ticket: a few microseconds when there is none).
         if (o.kernel == DSP_KERNEL_STAGE && getenv("DSP_LONG_NO_RETRY")) return 0;       // experiments only
         K.retry_only = 1;
@@ -1353,8 +1355,7 @@ static int solve_batch_host_locked(dsp_template *T, int64_t N, const double *cpa
     const bool ws_template = band_geometry(T, K).ws || (T->has_stage && T->sp.T > kStage2MaxT);    // (the long stage kernel's workspace too)
     // Chunks pay when there is something to overlap: the staging memcpy of pageable input (always), or the H2D copy of a batch whose
     // kernel runs for many waves.  A page-locked batch of a few waves goes in ONE piece: the persistent stage kernels fill every SM
-    // with one CTA, so two chunk kernels cannot share the chip and each chunk ends in its own thinning tail (C2 from pinned
-    // buffers: 0.665 ms in two chunks of 5 000 LPs, ~0.60 ms in one -- H2D 1.9 MB + 0.535 ms kernel + D2H).
+    // with one CTA, so two chunk kernels cannot share the chip and each chunk ends in its own thinning tail.
     const int nchunk = ws_template ? 1
                      : in_pinned   ? (int)std::min<int64_t>(4, std::max<int64_t>(1, N / 65536))
                                    : (int)std::min<int64_t>(8, std::max<int64_t>(1, N / 2048));

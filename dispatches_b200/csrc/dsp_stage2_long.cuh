@@ -623,7 +623,7 @@ __device__ void warp_body_long(const LongParams &LQ, int warp_global, int lane) 
             // second attempt: shorter step and a 100x proximal term (the other kernels use 10x).  At T = 8736 the failures are LPs whose
             // normal matrix (cond > 1e15) lets the solve drift along near-null directions: dx = D (A' dy - h) with D = x / z ~ 1e9 turns a
             // 1e-9 error of A' dy into a step of order 1, which the proximal term converts into a dual residual stuck at 1e-7; 1e-6
-            // damps that (emulator and B200: the one LP in 64 of the full-year sweep that 10x leaves NUMERICAL converges, 43 + 55
+            // damps that (on the emulator: the one LP in 64 of the full-year sweep that 10x leaves NUMERICAL converges, 43 + 55
             // iterations, objective 4e-12 from the band kernel's; 1000x stalls at MAX_ITER)
             const double sf = attempt ? 0.99 : LQ.q.step_frac, rg = attempt ? 100.0 * LQ.q.reg : LQ.q.reg;
             const int r = solve_long(LQ, wsw, (long long)t, lane, sf, rg, it0);

@@ -4,7 +4,7 @@
 // (wind_battery_LMP.py:172-267) in the reduced form of dispatches_b200/templates.py::wind_battery.
 //
 // Mapping: ONE WARP PER LP, ONE LANE PER PERIOD, STATE IN REGISTERS (no shared memory; ptxas spills ~0.4 KB per thread
-// to local memory at the 168-register cap -- ncu r1: 9.4 M LDL + 7.7 M STL per 10 000-LP launch):
+// to local memory at the 168-register cap):
 //   lane t holds the period's 7 columns  g (grid), i (charge), o (discharge), s (state of charge), e (throughput),
 //   p (slack of the SoC bound), q (slack of the wind balance), their duals, the 4 row duals and the Newton data.
 //   Neighbouring periods talk through warp shuffles (s[t-1], e[t-1], y1[t+1], y2[t+1]).
@@ -38,7 +38,7 @@ __device__ __forceinline__ double frcp(double x) {
     return r;
 }
 
-// max without fmax's NaN bookkeeping (DSETP.MAX + quiet-NaN fix-up costs ~9 SASS instructions per call, ncu r1)
+// max without fmax's NaN bookkeeping (DSETP.MAX + quiet-NaN fix-up costs ~9 SASS instructions per call)
 __device__ __forceinline__ double dmax(double a, double b) { return a > b ? a : b; }
 
 __device__ __forceinline__ double shfl_src(double v, int src) { return __shfl_sync(0xffffffffu, v, src); }
@@ -174,8 +174,8 @@ struct Out {
 };
 
 // solves LP number p; all 32 lanes of the warp participate.  The sweep loops are deliberately NOT unrolled and the horizon
-// is a run-time value: the iteration body is ~3k instructions, and a T=24 instantiation with unrolled sweeps (7k) ran 5 %
-// slower -- instruction-cache misses were 18 % of the stall samples (profiles/stage_variants_r1.log)
+// is a run-time value: the iteration body is ~3k instructions, and a T=24 instantiation with unrolled sweeps (7k) ran
+// slower, limited by instruction-cache misses
 __device__ int solve_one(const StageParams &S, const double *cp, const double *rpar, double kconst, long long p,
                           double tol, double feas_tol, double step_frac, double reg, int max_iter, const Out &O, int lane, int it0 PARK_PARAM) {
     const int T = S.T;

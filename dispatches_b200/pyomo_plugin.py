@@ -162,6 +162,6 @@ class B200IPM:
 
 if HAVE_PYOMO:                                  # pragma: no cover
     try:
-        SolverFactory.register("b200ipm", doc="B200 batched interior-point LP solver")(B200IPM)
+        SolverFactory.register("b200ipm", doc="H100 batched interior-point LP solver")(B200IPM)
     except Exception:                           # noqa: BLE001
         pass

@@ -497,8 +497,8 @@ def solar_battery_hydrogen(T: int, batt_mw=0.0, batt_mwh=0.0, pem_mw=0.0, tank_k
     B.obj_const((1e-3 * (cap + PA * fixed), {iPV: 1e-3 * PA * P["pv_op_cost"]}))
     # The reference sizes the tank EXACTLY for the reserve it must back (inputs.py:86): at night turbine_reserve >= reserve forces the
     # holdup to its upper bound, the feasible set has no strict interior in those columns and the interior-point iterates crawl
-    # (114 iterations for 1 LP in 256 with the default proximal term 1e-8; <= 15 for all with 1e-7, measured on the B200:
-    # tools/gpu_solar_diag.py) -- the solver reads this value unless the caller passes its own.
+    # (with the default proximal term 1e-8 an occasional LP needs over 100 iterations, with 1e-7 none needs more than about 15:
+    # tools/gpu_solar_diag.py compares the two) -- the solver reads this value unless the caller passes its own.
     B.meta.update(kind="solar_battery_hydrogen", T=T, ann=ann, capital_cost=cap, k_turb=k_turb, tank_kg=tank_kg,
                   sizes=dict(batt_kw=Bc, batt_kwh=Be, pem_kw=Pc, turb_kw=Tc), reg_primal=1e-7)
     return B.build(equilibrate=True)         # holdups (1e6 mol) next to powers (1e5 kW) and flows (1e2 mol/s)

@@ -1,5 +1,5 @@
 /*
- * dsp_lp.h -- C ABI of the B200 batched dispatch-LP solver (libdsp_lp.so).
+ * dsp_lp.h -- C ABI of the H100 batched dispatch-LP solver (libdsp_lp.so).
  *
  * The reference (gmlc-dispatches/dispatches) is pure Python and has no FFI; the boundary this library
  * sits behind is Pyomo's solver-plugin call
@@ -113,7 +113,7 @@ int dsp_lp_template_set_stage_chain1(dsp_template *t, const dsp_stage_chain1_des
  * the complementarity gap has converged (< tol) while residuals / gap sit at the rounding floor of the ill-conditioned normal
  * equations, residuals < 10 feas_tol and gap < 10 tol; OR complementarity < 1e-3 tol with residuals < 100 feas_tol and
  * gap < 1000 tol (the effective worst-case tolerance is therefore 1000 tol = 1e-6 relative on the LP part of the objective at
- * the defaults; measured worst case on the 560 640 LPs of config C5: 3e-8).  DSP_INFEASIBLE is reported only for a negative
+ * the defaults).  DSP_INFEASIBLE is reported only for a negative
  * upper bound produced by Umap / rparams (obj = NaN); other infeasible / unbounded LPs end as DSP_MAX_ITER / DSP_NUMERICAL. */
 enum { DSP_OPTIMAL = 0, DSP_MAX_ITER = 1, DSP_NUMERICAL = 2, DSP_INFEASIBLE = 3 };
 enum { DSP_E_ARG = -1, DSP_E_CUDA = -2, DSP_E_SMEM = -3, DSP_E_BUSY = -4 /* a host call is already in flight on this handle */ };

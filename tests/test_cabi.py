@@ -22,11 +22,11 @@ def test_library_exports_every_declared_symbol(cuda_solver_lib):
     for name in declared_functions():
         assert hasattr(cuda_solver_lib, name), name
     assert sorted(solver.EXPORTS) == declared_functions()
-    assert b"sm_100a" in cuda_solver_lib.dsp_lp_version()
+    assert b"sm_90a" in cuda_solver_lib.dsp_lp_version()
 
 
-def test_sass_is_sm100a_with_tma_staging():
-    """The built library carries sm_100a SASS with the TMA bulk copy (UBLKCP) and FP64 FMAs."""
+def test_sass_is_sm90a_with_tma_staging():
+    """The built library carries sm_90a SASS with the TMA bulk copy (UBLKCP) and FP64 FMAs."""
     import shutil
     import subprocess
     if shutil.which("cuobjdump") is None:
@@ -35,7 +35,7 @@ def test_sass_is_sm100a_with_tma_staging():
     from dispatches_b200.csrc import build
     lib = build.build()
     sass = subprocess.run(["cuobjdump", "-sass", str(lib)], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass and "UBLKCP" in sass and "DFMA" in sass
+    assert "sm_90a" in sass and "UBLKCP" in sass and "DFMA" in sass
 
 
 def test_no_cpu_fallback_in_product():
@@ -72,8 +72,8 @@ def test_argument_errors_are_reported_without_a_gpu(cuda_solver_lib):
 
 
 def test_forced_rebuild_from_source():
-    """build(force=True) recompiles libdsp_lp.so from the sources for sm_100a (nvcc cross-compiles without a GPU) -- the
-    round-end check must not depend on a stale prebuilt library."""
+    """build(force=True) recompiles libdsp_lp.so from the sources for sm_90a (nvcc cross-compiles without a GPU): a check
+    of the tree must not depend on a stale prebuilt library."""
     import time
     from dispatches_b200.csrc import build
     t0 = time.time()

@@ -1,4 +1,4 @@
-"""Turns the ncu artefacts in gpurun_out/ into small tracked summaries under profiles/ (run here, no GPU)."""
+"""Turns the ncu captures and launch CSVs the tools/ scripts wrote into small summaries under profiles/ (git-ignored; needs no GPU)."""
 import csv, collections, json, subprocess, sys
 from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
