@@ -473,11 +473,6 @@ __global__ void __launch_bounds__(kMaxWarps * 32, 1) dsp_ipm_band_kernel(const K
     if (WS && P.hybrid) band0 = (double *)(smem + P.prob_off) + (size_t)warp * P.band_doubles;
     W.dy = band0 + BW;
     W.Mb = W.dy + m + BW + BW * (BW + 1);
-#ifdef DSP_EXPERIMENT_HYBRID2
-    // round-2 experiment (tools/build_variants.py): the gather sources of the CSR product and of the assembly (dx, d) next
-    // to the band in shared memory; P.band_doubles then includes 2 n
-    if (WS && P.hybrid == 2) { W.dx = band0 + (P.band_doubles - 2 * n); W.d = W.dx + n; }
-#endif
     for (;;) {
         unsigned long long t = 0;
         if (lane == 0) t = atomicAdd(P.ticket, 1ULL);
@@ -497,13 +492,9 @@ namespace {
 #include "dsp_stage_wb.cuh"
 
 // stage kernel: one warp per LP, one lane per period, all state in registers (see dsp_stage_wb.cuh)
-#ifndef DSP_STAGE_MINB
-#define DSP_STAGE_MINB 3
-#endif
-#ifndef DSP_STAGE_WPB
-#define DSP_STAGE_WPB 4
-#endif
-__global__ void __launch_bounds__(32 * DSP_STAGE_WPB, DSP_STAGE_MINB) dsp_ipm_stage_wb_kernel(const KParams P, const stagewb::StageParams S) {
+constexpr int kStageWarps = 4;          // warps per CTA
+constexpr int kStageMinBlocks = 3;      // CTAs per SM the register allocation must allow
+__global__ void __launch_bounds__(32 * kStageWarps, kStageMinBlocks) dsp_ipm_stage_wb_kernel(const KParams P, const stagewb::StageParams S) {
     const int lane = threadIdx.x & 31;
     stagewb::Out O;
     O.obj = P.obj; O.x_out = P.x_out; O.y_out = P.y_out; O.status = P.status; O.iters = P.iters; O.n = P.n; O.m = P.m;
@@ -523,13 +514,7 @@ __global__ void __launch_bounds__(32 * DSP_STAGE_WPB, DSP_STAGE_MINB) dsp_ipm_st
         int it0 = 0;
         for (int attempt = 0; attempt < 2; ++attempt) {
             const double sf = attempt ? 0.99 : P.step_frac, rg = attempt ? 10.0 * P.reg : P.reg;
-#ifdef DSP_STAGE_PARK
-            __shared__ double park_all[DSP_STAGE_WPB][(DSP_STAGE_PARK >= 2 ? 40 : 22) * 32];
-            const int r = stagewb::solve_one(S, cp, rp, kconst, (long long)t, P.tol, P.feas_tol, sf, rg, P.max_iter, O, lane, it0,
-                                             park_all[threadIdx.x >> 5] + lane);
-#else
             const int r = stagewb::solve_one(S, cp, rp, kconst, (long long)t, P.tol, P.feas_tol, sf, rg, P.max_iter, O, lane, it0);
-#endif
             if (r == 0) break;
             it0 = r - 1;
         }
@@ -543,20 +528,17 @@ __global__ void __launch_bounds__(32 * DSP_STAGE_WPB, DSP_STAGE_MINB) dsp_ipm_st
 namespace {
 // stage kernel, generation 2: 32/L LPs per warp, P periods per lane, one warp per CTA (see dsp_stage2.cuh).  The register
 // budget is the full 255 (65536 / (7 CTAs x 32 threads) = 292): occupancy is set by the 31 KB of shared memory per warp.
-#ifndef DSP_S2_WARPS
-#define DSP_S2_WARPS 8
-#endif
-constexpr int kStage2Warps = DSP_S2_WARPS;        // warps per CTA = per SM: 8 x 27.9 KB of shared memory, 8 x 32 x 255 registers.  (A ninth
-                                                 // warp does not fit the register file, which is per scheduler: a third warp on one of the
-                                                 // four caps every thread at 168 registers -- 2 KB of spills)
+constexpr int kStage2Warps = 8;     // warps per CTA = per SM: 8 x 27.9 KB of shared memory, 8 x 32 x 255 registers.  (A ninth
+                                    // warp does not fit the register file, which is per scheduler: a third warp on one of the
+                                    // four caps every thread at 168 registers -- 2 KB of spills)
 // warps per CTA (= per SM) of the chain kernel: what shared memory allows at 168 registers per thread (three warps on a scheduler).
 // NF = 2 (19.5 KB per warp): 11 warps -- 2 904 group slots at L = 16 on the 132 SMs of an H100, so the 5 000 LPs of C3 are two
 // waves instead of the three they are at 8 warps / 219 registers; NF = 3 (24.8 KB per warp): 8
 constexpr int chain1_warps(int NF) { return NF == 2 ? 11 : 8; }
-template <int L, int P, bool SYNC>
+template <int L, int P>
 __global__ void __launch_bounds__(32 * kStage2Warps, 1) dsp_ipm_stage2_wb_kernel(const stage2::Params Q) {
     extern __shared__ __align__(16) double s2_smem[];
-    stage2::warp_body<L, P, SYNC>(Q, s2_smem + (threadIdx.x >> 5) * stage2::SmemDoubles<P>::value, threadIdx.x & 31);
+    stage2::warp_body<L, P>(Q, s2_smem + (threadIdx.x >> 5) * stage2::SmemDoubles<P>::value, threadIdx.x & 31);
 }
 
 }  // namespace
@@ -569,7 +551,7 @@ namespace {
 template <int L, int P, int NF>
 __global__ void __launch_bounds__(32 * chain1_warps(NF), 1) dsp_ipm_stage_chain1_kernel(const chain1::Params Q) {
     extern __shared__ __align__(16) double s2_smem[];
-    chain1::warp_body<L, P, NF, true>(Q, s2_smem + (threadIdx.x >> 5) * chain1::Smem<NF, P>::doubles_per_warp, threadIdx.x & 31);
+    chain1::warp_body<L, P, NF>(Q, s2_smem + (threadIdx.x >> 5) * chain1::Smem<NF, P>::doubles_per_warp, threadIdx.x & 31);
 }
 inline int chain1_lanes(int T) { return T <= 12 ? 4 : T <= 24 ? 8 : T <= 48 ? 16 : 32; }
 constexpr int kChain1MaxT = 96;
@@ -582,10 +564,6 @@ __global__ void __launch_bounds__(32 * kLongWarps) dsp_ipm_stage2_long_kernel(co
 
 struct Stage2Geom { int L, P; };
 inline Stage2Geom stage2_geometry(int T) {
-    if (const char *e = getenv("DSP_STAGE2_GEOM")) {       // experiments only: "L,P"
-        int l = 0, p = 0;
-        if (sscanf(e, "%d,%d", &l, &p) == 2 && l * p >= T && (p == 3 || (l == 16 && p == 2))) return {l, p};
-    }
     if (T <= 6) return {2, 3};
     if (T <= 12) return {4, 3};
     if (T <= 24) return {8, 3};
@@ -649,7 +627,6 @@ struct dsp_template {
     int c1_T, c1_NF;
     const int *c1_col_idx, *c1_row_idx;
     const double *c1_coef, *c1_coef_next;
-    int stage2_blocks_per_sm;      // generation-2 stage kernel: CTAs (= warps) per SM for this template's (L, P)
     int device;
     int sm_count;
     int smem_optin;
@@ -671,23 +648,55 @@ struct dsp_template {
 };
 
 namespace {
-#define S2_DISPATCH(CALL)                                                   \
-    do {                                                                    \
-        if (g.L == 2) { CALL(2, 3); }                                       \
-        else if (g.L == 4) { CALL(4, 3); }                                  \
-        else if (g.L == 8) { CALL(8, 3); }                                  \
-        else if (g.L == 16 && g.P == 2) { CALL(16, 2); }                    \
-        else if (g.L == 16) { CALL(16, 3); }                                \
-        else { CALL(32, 3); }                                               \
-    } while (0)
-const void *stage2_function(const Stage2Geom &g, bool sync) {
-#define S2_FN(l, p) return sync ? (const void *)dsp_ipm_stage2_wb_kernel<l, p, true> : (const void *)dsp_ipm_stage2_wb_kernel<l, p, false>
-    S2_DISPATCH(S2_FN);
-#undef S2_FN
-    return nullptr;
+// The kernel instantiation of each family for a geometry.  Launches and cudaFuncSetAttribute calls both look it up here.
+using BandKernel = void (*)(KParams);
+using Stage2Kernel = void (*)(stage2::Params);
+using Chain1Kernel = void (*)(chain1::Params);
+
+// band kernel for half bandwidth W and a placement: work regions in the global workspace (ws) or in shared memory, with the
+// template staged into shared memory (hot_in_smem) or read through L2
+template <int W>
+BandKernel band_kernel_w(bool ws, bool hot_in_smem) {
+    return ws ? dsp_ipm_band_kernel<W, true, false> : hot_in_smem ? dsp_ipm_band_kernel<W, false, true> : dsp_ipm_band_kernel<W, false, false>;
+}
+BandKernel band_kernel(int w, bool ws, bool hot_in_smem) {
+    switch (w) {
+        case 1: return band_kernel_w<1>(ws, hot_in_smem);
+        case 2: return band_kernel_w<2>(ws, hot_in_smem);
+        case 4: return band_kernel_w<4>(ws, hot_in_smem);
+        case 8: return band_kernel_w<8>(ws, hot_in_smem);
+        case 16: return band_kernel_w<16>(ws, hot_in_smem);
+        default: return band_kernel_w<32>(ws, hot_in_smem);
+    }
+}
+
+Stage2Kernel stage2_kernel(const Stage2Geom &g) {
+    if (g.L == 2) return dsp_ipm_stage2_wb_kernel<2, 3>;
+    if (g.L == 4) return dsp_ipm_stage2_wb_kernel<4, 3>;
+    if (g.L == 8) return dsp_ipm_stage2_wb_kernel<8, 3>;
+    if (g.L == 16) return g.P == 2 ? dsp_ipm_stage2_wb_kernel<16, 2> : dsp_ipm_stage2_wb_kernel<16, 3>;
+    return dsp_ipm_stage2_wb_kernel<32, 3>;
 }
 size_t stage2_smem_bytes(const Stage2Geom &g) {
     return (size_t)(g.P == 2 ? stage2::smem_doubles_per_warp<2>() : stage2::smem_doubles_per_warp<3>()) * 8;
+}
+
+template <int NF>
+Chain1Kernel chain1_kernel_nf(int L) {
+    return L == 4 ? dsp_ipm_stage_chain1_kernel<4, 3, NF> : L == 8 ? dsp_ipm_stage_chain1_kernel<8, 3, NF>
+         : L == 16 ? dsp_ipm_stage_chain1_kernel<16, 3, NF> : dsp_ipm_stage_chain1_kernel<32, 3, NF>;
+}
+Chain1Kernel chain1_kernel(int L, int NF) { return NF == 2 ? chain1_kernel_nf<2>(L) : chain1_kernel_nf<3>(L); }
+size_t chain1_smem_bytes(int NF) {
+    return (size_t)(NF == 2 ? chain1::Smem<2, 3>::doubles_per_warp : chain1::Smem<3, 3>::doubles_per_warp) * 8;
+}
+
+// lets a stage kernel use `bytes` of dynamic shared memory, with the largest carveout
+template <class F>
+int allow_smem(F fn, size_t bytes) {
+    CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    CK(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    return 0;
 }
 }  // namespace
 
@@ -819,7 +828,7 @@ int dsp_lp_template_create(const dsp_template_desc *D, dsp_template **out) {
     } guard{T};
     memset(&T->kp, 0, sizeof(KParams));
     T->cap_N = 0; T->cap_x = T->cap_y = false; T->cap_rp_rows = 0;
-    T->has_stage = false; T->has_chain1 = false; T->stage_blocks_per_sm = 0; T->stage2_blocks_per_sm = 0; T->ws = nullptr; T->ws_bytes = 0;
+    T->has_stage = false; T->has_chain1 = false; T->stage_blocks_per_sm = 0; T->ws = nullptr; T->ws_bytes = 0;
     T->h_cp = T->h_rp = T->h_obj = T->h_x = T->h_y = nullptr; T->h_status = T->h_iters = nullptr;
     T->d_cp = T->d_rp = T->d_obj = T->d_x = T->d_y = nullptr; T->d_status = T->d_iters = nullptr;
     T->stream = nullptr; T->stream2 = nullptr; T->busy.store(0);
@@ -879,24 +888,9 @@ int dsp_lp_template_create(const dsp_template_desc *D, dsp_template **out) {
     K.band_doubles = (m + 2 * wt) + (m + 2 * wt) * (wt + 1);
     K.prob_doubles = 8 * n + 6 * nb + 3 * m + K.band_doubles;
     K.hybrid = 0;
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<1, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<1, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<2, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<4, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<4, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<8, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<8, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<16, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<16, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<1, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<2, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<4, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<8, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<16, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<32, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<32, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaFuncSetAttribute(dsp_ipm_band_kernel<32, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
+    for (int bw = 1; bw <= 32; bw *= 2)
+        for (int placement = 0; placement < 3; ++placement)       // workspace, shared memory + staged template, shared memory
+            CK(cudaFuncSetAttribute(band_kernel(bw, placement == 0, placement == 1), cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
     CK(cudaStreamCreateWithFlags(&T->stream, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&T->stream2, cudaStreamNonBlocking));
     guard.t = nullptr;
@@ -922,17 +916,12 @@ int dsp_lp_template_set_stage_wb(dsp_template *T, const dsp_stage_wb_desc *d) {
     T->dev_allocs.push_back(dci); T->dev_allocs.push_back(dri);
     S.col_idx = dci; S.row_idx = dri;
     int nb = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, dsp_ipm_stage_wb_kernel, 32 * DSP_STAGE_WPB, 0));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, dsp_ipm_stage_wb_kernel, 32 * kStageWarps, 0));
     T->stage_blocks_per_sm = std::max(nb, 1);
     if (d->T <= kStage2MaxT) {
         const Stage2Geom g = stage2_geometry(d->T);
-        const size_t smem = stage2_smem_bytes(g) * kStage2Warps;
-        for (int sync = 0; sync < 2; ++sync) {
-            const void *fn = stage2_function(g, sync != 0);
-            CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            CK(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-        }
-        T->stage2_blocks_per_sm = 1;
+        rc = allow_smem(stage2_kernel(g), stage2_smem_bytes(g) * kStage2Warps);
+        if (rc) return rc;
     }
     T->has_stage = true;
     return 0;
@@ -967,13 +956,8 @@ int dsp_lp_template_set_stage_chain1(dsp_template *T, const dsp_stage_chain1_des
     rc = upload(cn, &dcn); if (rc) return rc; T->dev_allocs.push_back(dcn);
     T->c1_T = d->T; T->c1_NF = d->NF;
     T->c1_col_idx = dci; T->c1_row_idx = dri; T->c1_coef = dcf; T->c1_coef_next = dcn;
-    const int L = chain1_lanes(d->T);
-    const size_t smem = (size_t)(T->c1_NF == 2 ? chain1::Smem<2, 3>::doubles_per_warp : chain1::Smem<3, 3>::doubles_per_warp) * 8 * chain1_warps(T->c1_NF);
-#define C1_ATTR(l, nf) do { CK(cudaFuncSetAttribute(dsp_ipm_stage_chain1_kernel<l, 3, nf>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-                            CK(cudaFuncSetAttribute(dsp_ipm_stage_chain1_kernel<l, 3, nf>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared)); } while (0)
-    if (T->c1_NF == 2) { if (L == 4) C1_ATTR(4, 2); else if (L == 8) C1_ATTR(8, 2); else if (L == 16) C1_ATTR(16, 2); else C1_ATTR(32, 2); }
-    else { if (L == 4) C1_ATTR(4, 3); else if (L == 8) C1_ATTR(8, 3); else if (L == 16) C1_ATTR(16, 3); else C1_ATTR(32, 3); }
-#undef C1_ATTR
+    rc = allow_smem(chain1_kernel(chain1_lanes(d->T), d->NF), chain1_smem_bytes(d->NF) * chain1_warps(d->NF));
+    if (rc) return rc;
     T->has_chain1 = true;
     return 0;
 }
@@ -999,12 +983,7 @@ struct BandGeom { long long warps; int hot_in_smem; size_t off; bool ws; int hyb
 
 BandGeom band_geometry(const dsp_template *T, const KParams &K) {
     const size_t prob_bytes = (size_t)K.prob_doubles * 8;
-    size_t band_bytes = (size_t)K.band_doubles * 8;
-#ifdef DSP_EXPERIMENT_HYBRID2
-    const char *h2 = getenv("DSP_BAND_MODE");
-    const bool hybrid2 = h2 && !strcmp(h2, "hybrid2");
-    if (hybrid2) band_bytes += (size_t)2 * K.n * 8;
-#endif
+    const size_t band_bytes = (size_t)K.band_doubles * 8;
     const size_t budget = (size_t)T->smem_optin;
     BandGeom g{0, 1, 16 + (size_t)K.hot_bytes, false, 0};
     long long smem_warps = budget > g.off ? (long long)((budget - g.off) / prob_bytes) : 0;
@@ -1015,27 +994,157 @@ BandGeom band_geometry(const dsp_template *T, const KParams &K) {
     }
     const long long hybrid_warps = band_bytes + 16 <= budget ? std::min<long long>(kMaxWarps, (long long)((budget - 16) / band_bytes)) : 0;
     enum { M_SMEM, M_HYBRID, M_WS } mode = smem_warps >= 7 ? M_SMEM : hybrid_warps >= 6 ? M_HYBRID : smem_warps >= 4 ? M_SMEM : M_WS;
-    if (const char *e = getenv("DSP_BAND_MODE")) {            // experiment switch
+#ifdef DSP_PHASES
+    // instrumentation build only: tools/gpu_band_modes.py forces a placement (DSP_BAND_MODE = smem | hybrid | ws) where it fits
+    if (const char *e = getenv("DSP_BAND_MODE")) {
         if (!strcmp(e, "ws")) mode = M_WS;
         else if (!strcmp(e, "hybrid") && hybrid_warps >= 1) mode = M_HYBRID;
-#ifdef DSP_EXPERIMENT_HYBRID2
-        else if (hybrid2 && hybrid_warps >= 1) mode = M_HYBRID;
-#endif
         else if (!strcmp(e, "smem") && smem_warps >= 1) mode = M_SMEM;
     }
+#endif
     if (mode == M_SMEM) {
         g.warps = smem_warps;
     } else {
         g.ws = true; g.hot_in_smem = 0; g.off = 16;
         g.hybrid = mode == M_HYBRID;
-#ifdef DSP_EXPERIMENT_HYBRID2
-        if (g.hybrid && hybrid2) g.hybrid = 2;
-#endif
         g.warps = g.hybrid ? hybrid_warps : kMaxWarps;
         while (g.warps > 1 && (size_t)T->sm_count * (size_t)g.warps * prob_bytes > T->ws_cap) g.warps /= 2;
     }
     g.warps = std::min<long long>(g.warps, kMaxWarps);
     return g;
+}
+
+// grows the handle's global workspace to at least `need` bytes, once the kernels already queued on the stream are done with it
+static int grow_ws(const dsp_template *T, size_t need, cudaStream_t st) {
+    if (need <= T->ws_bytes) return 0;
+    CK(cudaStreamSynchronize(st));
+    cudaFree(T->ws);
+    T->ws = nullptr; T->ws_bytes = 0;
+    CK(cudaMalloc((void **)&T->ws, need));
+    T->ws_bytes = need;
+    return 0;
+}
+
+// checks the launch just issued and records its geometry for dsp_lp_launch_count / dsp_lp_last_launch
+static int launched(long long grid, long long block, size_t smem, long long ppc) {
+    CK(cudaGetLastError());
+    std::lock_guard<std::mutex> lk(g_mu);
+    g_launches++;
+    g_last_grid = (int)grid; g_last_block = (int)block; g_last_smem = (int)smem; g_last_ppc = (int)ppc;
+    return 0;
+}
+
+// parameters of the stage-2 kernels (short and long horizon): the batch in K, the stage structure of the template
+static stage2::Params stage2_params(const dsp_template *T, const KParams &K) {
+    stage2::Params Q;
+    Q.N = K.N; Q.cparams = K.cparams; Q.rparams = K.rparams; Q.rstride = K.rstride; Q.Pc = K.Pc; Q.Pr = K.Pr;
+    Q.omap = K.omap; Q.ocmap = K.ocmap; Q.o0 = K.o0;
+    Q.tol = K.tol; Q.feas_tol = K.feas_tol; Q.step_frac = K.step_frac; Q.reg = K.reg; Q.max_iter = K.max_iter;
+    Q.obj = K.obj; Q.x_out = K.x_out; Q.y_out = K.y_out; Q.status = K.status; Q.iters = K.iters; Q.n = K.n; Q.m = K.m; Q.ticket = K.ticket;
+    const stagewb::StageParams &S = T->sp;
+    Q.T = S.T; Q.a = S.a; Q.binv = S.binv; Q.hf = S.hf; Q.dl = S.dl; Q.dur = S.dur; Q.krev = S.krev;
+    Q.wcf_off = S.wcf_off; Q.p_off = S.p_off; Q.col_idx = S.col_idx; Q.row_idx = S.row_idx;
+    Q.ahead = 0;
+    return Q;
+}
+
+// long horizon (T > 96): one warp per LP, everything in a global workspace owned by the handle
+static int launch_stage2_long(const dsp_template *T, const KParams &K, cudaStream_t st) {
+    const int P = (T->sp.T + 31) / 32;
+    const size_t per_warp = (size_t)stage2long::NW * P * 32 * sizeof(double);
+    int occ = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dsp_ipm_stage2_long_kernel, 32 * kLongWarps, 0));
+    long long warps = std::min<long long>(K.N, (long long)T->sm_count * std::max(occ, 1) * kLongWarps);
+    while (warps > 1 && (size_t)warps * per_warp > T->ws_cap) warps /= 2;
+    // spread the warps over the SMs: one warp per CTA while there are fewer LPs than SMs x kLongWarps
+    const int wpb = (int)std::min<long long>(kLongWarps, std::max<long long>(1, warps / T->sm_count));
+    const long long blocks = (warps + wpb - 1) / wpb;
+    const int rc = grow_ws(T, (size_t)blocks * wpb * per_warp, st);
+    if (rc) return rc;
+    stage2long::LongParams LQ;
+    LQ.q = stage2_params(T, K);
+    LQ.ws = T->ws; LQ.P = P;
+    CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
+    dsp_ipm_stage2_long_kernel<<<(unsigned)blocks, 32 * wpb, 0, st>>>(LQ);
+    return launched(blocks, 32 * wpb, 0, wpb);
+}
+
+// generation-2 stage kernel: 32/L LPs per warp, persistent CTAs, LP groups refill from the ticket counter
+static int launch_stage2(const dsp_template *T, const KParams &K, cudaStream_t st) {
+    const Stage2Geom g = stage2_geometry(T->sp.T);
+    const int per_warp = 32 / g.L;
+    // one persistent CTA per SM; its warps (up to kStage2Warps) run the phases of an IPM round in step
+    int wmax = kStage2Warps;
+#ifdef DSP_PHASES
+    // instrumentation build only: tools/gpu_stage2_phases.py compares fewer warps per CTA (DSP_STAGE2_WARPS)
+    if (const char *e = getenv("DSP_STAGE2_WARPS")) wmax = std::min(kStage2Warps, std::max(1, atoi(e)));
+#endif
+    const long long warps_needed = (K.N + per_warp - 1) / per_warp;
+    const long long blocks = std::max<long long>(1, std::min<long long>(T->sm_count, warps_needed));
+    const int wpb = (int)std::min<long long>(wmax, (warps_needed + blocks - 1) / blocks);
+    const size_t smem = stage2_smem_bytes(g) * wpb;
+    stage2::Params Q = stage2_params(T, K);
+    Q.ahead = (int)(blocks * wpb * per_warp);
+    CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
+    stage2_kernel(g)<<<(unsigned)blocks, 32 * wpb, smem, st>>>(Q);
+    return launched(blocks, 32 * wpb, smem, per_warp * wpb);
+}
+
+// generation-1 stage kernel (lane per period): no shared memory; persistent warps, one LP per warp at a time
+static int launch_stage_v1(const dsp_template *T, const KParams &K, cudaStream_t st) {
+    if (T->sp.T > 32) { g_err = "dsp_lp_solve_batch: the lane-per-period stage kernel needs T <= 32"; return DSP_E_ARG; }
+    const long long blocks = std::min<long long>((long long)T->sm_count * T->stage_blocks_per_sm, (K.N + kStageWarps - 1) / kStageWarps);
+    CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
+    dsp_ipm_stage_wb_kernel<<<(unsigned)blocks, kStageWarps * 32, 0, st>>>(K, T->sp);
+    return launched(blocks, kStageWarps * 32, 0, kStageWarps);
+}
+
+// descriptor-driven single-storage-chain stage kernel: the CTA shape of stage 2, chain1_warps(NF) warps at most
+static int launch_chain1(const dsp_template *T, const KParams &K, cudaStream_t st) {
+    const int L = chain1_lanes(T->c1_T), per_warp = 32 / L, NF = T->c1_NF;
+    const long long warps_needed = (K.N + per_warp - 1) / per_warp;
+    const long long blocks = std::max<long long>(1, std::min<long long>(T->sm_count, warps_needed));
+    const int wpb = (int)std::min<long long>(chain1_warps(NF), (warps_needed + blocks - 1) / blocks);
+    const size_t smem = chain1_smem_bytes(NF) * wpb;
+    chain1::Params Q;
+    Q.N = K.N; Q.cparams = K.cparams; Q.rparams = K.rparams; Q.rstride = K.rstride; Q.Pc = K.Pc; Q.Pr = K.Pr;
+    Q.omap = K.omap; Q.ocmap = K.ocmap; Q.o0 = K.o0;
+    Q.tol = K.tol; Q.feas_tol = K.feas_tol; Q.step_frac = K.step_frac; Q.reg = K.reg; Q.max_iter = K.max_iter;
+    Q.obj = K.obj; Q.x_out = K.x_out; Q.y_out = K.y_out; Q.status = K.status; Q.iters = K.iters; Q.n = K.n; Q.m = K.m; Q.nb = K.nb; Q.ticket = K.ticket;
+    Q.c0 = K.c0; Q.b0 = K.b0; Q.u0 = K.u0; Q.cm_ptr = K.cm_ptr; Q.cm_idx = K.cm_idx; Q.cm_val = K.cm_val;
+    Q.bm_ptr = K.bm_ptr; Q.bm_idx = K.bm_idx; Q.bm_val = K.bm_val; Q.um_ptr = K.um_ptr; Q.um_idx = K.um_idx; Q.um_val = K.um_val;
+    Q.T = T->c1_T; Q.col_idx = T->c1_col_idx; Q.row_idx = T->c1_row_idx; Q.coef = T->c1_coef; Q.coef_next = T->c1_coef_next;
+    Q.x_perm = K.xperm; Q.y_perm = K.yperm;
+    CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
+    chain1_kernel(L, NF)<<<(unsigned)blocks, 32 * wpb, smem, st>>>(Q);
+    return launched(blocks, 32 * wpb, smem, per_warp * wpb);
+}
+
+// generic band kernel, in the placement band_geometry picks
+static int launch_band(const dsp_template *T, KParams K, cudaStream_t st) {
+    const size_t prob_bytes = (size_t)K.prob_doubles * 8;
+    const BandGeom geom = band_geometry(T, K);
+    long long warps = geom.warps;
+    long long ctas = std::min<long long>(T->sm_count, (K.N + warps - 1) / warps);
+    // spread a small batch over all SMs
+    if (ctas < T->sm_count && K.N > ctas) {
+        ctas = std::min<long long>(T->sm_count, K.N);
+        warps = std::min<long long>(warps, (K.N + ctas - 1) / ctas);
+    }
+    K.hot_in_smem = geom.hot_in_smem;
+    K.prob_off = (int)geom.off;
+    K.ws = nullptr;
+    K.hybrid = geom.hybrid;
+    size_t smem = geom.off + (size_t)warps * prob_bytes;
+    if (geom.ws) {
+        const int rc = grow_ws(T, (size_t)ctas * (size_t)warps * prob_bytes, st);
+        if (rc) return rc;
+        K.ws = T->ws;
+        smem = geom.hybrid ? geom.off + (size_t)warps * K.band_doubles * 8 : 16;
+    }
+    CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
+    band_kernel(K.w, geom.ws, geom.hot_in_smem)<<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
+    return launched(ctas, warps * 32, smem, warps);
 }
 
 static int launch_batch(const dsp_template *T, int64_t N, const double *cparams, const double *rparams,
@@ -1056,199 +1165,25 @@ static int launch_batch(const dsp_template *T, int64_t N, const double *cparams,
     K.obj = obj; K.status = status; K.iters = iters; K.x_out = x; K.y_out = y;
     K.ticket = ticket;
     K.retry_only = 0;
-    if (T->has_stage && T->sp.T > kStage2MaxT && (o.kernel == DSP_KERNEL_AUTO || o.kernel == DSP_KERNEL_STAGE)) {
-        // long horizon: one warp per LP, everything in a global workspace owned by the handle
-        const int P = (T->sp.T + 31) / 32;
-        const size_t per_warp = (size_t)stage2long::NW * P * 32 * sizeof(double);
-        int occ = 0;
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dsp_ipm_stage2_long_kernel, 32 * kLongWarps, 0));
-        long long warps = std::min<long long>(N, (long long)T->sm_count * std::max(occ, 1) * kLongWarps);
-        while (warps > 1 && (size_t)warps * per_warp > T->ws_cap) warps /= 2;
-        // spread the warps over the SMs: one warp per CTA while there are fewer LPs than SMs x kLongWarps
-        const int wpb = (int)std::min<long long>(kLongWarps, std::max<long long>(1, warps / T->sm_count));
-        const long long blocks = (warps + wpb - 1) / wpb;
-        const size_t need = (size_t)blocks * wpb * per_warp;
-        if (need > T->ws_bytes) {
-            CK(cudaStreamSynchronize(st));
-            cudaFree(T->ws);
-            T->ws = nullptr; T->ws_bytes = 0;
-            CK(cudaMalloc((void **)&T->ws, need));
-            T->ws_bytes = need;
-        }
-        stage2long::LongParams LQ;
-        stage2::Params &Q = LQ.q;
-        Q.N = N; Q.cparams = cparams; Q.rparams = rparams; Q.rstride = rparams_stride; Q.Pc = K.Pc; Q.Pr = K.Pr;
-        Q.omap = K.omap; Q.ocmap = K.ocmap; Q.o0 = K.o0;
-        Q.tol = o.tol; Q.feas_tol = o.feas_tol; Q.step_frac = o.step_frac; Q.reg = o.reg_primal; Q.max_iter = o.max_iter;
-        Q.obj = obj; Q.x_out = x; Q.y_out = y; Q.status = status; Q.iters = iters; Q.n = K.n; Q.m = K.m; Q.ticket = ticket;
-        const stagewb::StageParams &S = T->sp;
-        Q.T = S.T; Q.a = S.a; Q.binv = S.binv; Q.hf = S.hf; Q.dl = S.dl; Q.dur = S.dur; Q.krev = S.krev;
-        Q.wcf_off = S.wcf_off; Q.p_off = S.p_off; Q.col_idx = S.col_idx; Q.row_idx = S.row_idx;
-        Q.ahead = 0;
-        LQ.ws = T->ws; LQ.P = P;
-        CK(cudaMemsetAsync(ticket, 0, sizeof(unsigned long long), st));
-        dsp_ipm_stage2_long_kernel<<<(unsigned)blocks, 32 * wpb, 0, st>>>(LQ);
-        CK(cudaGetLastError());
-        {
-            std::lock_guard<std::mutex> lk(g_mu);
-            g_launches++;
-            g_last_grid = (int)blocks; g_last_block = 32 * wpb; g_last_smem = 0; g_last_ppc = wpb;
-        }
+    const bool stage = o.kernel == DSP_KERNEL_AUTO || o.kernel == DSP_KERNEL_STAGE;
+    if (T->has_stage && T->sp.T > kStage2MaxT && stage) {
+        const int rc = launch_stage2_long(T, K, st);
+        if (rc) return rc;
         // At T = 8736 cond(M) reaches 1e15 and the partitioned elimination order rounds differently from the band kernel's
-        // sequential one: about 1 LP in 60 of the reference's full-year sweep stalls here and converges there.
-        // The band kernel therefore follows on the same stream and re-solves ONLY the LPs this
-        // kernel left with MAX_ITER / NUMERICAL (its warps skip every other ticket: a few microseconds when there is none).
-        if (o.kernel == DSP_KERNEL_STAGE && getenv("DSP_LONG_NO_RETRY")) return 0;       // experiments only
+        // sequential one: about 1 LP in 60 of the reference's full-year sweep stalls in the long kernel and converges in the
+        // band kernel.  The band kernel therefore follows on the same stream and re-solves ONLY the LPs the long kernel left
+        // with MAX_ITER / NUMERICAL (its warps skip every other ticket: a few microseconds when there is none).
         K.retry_only = 1;
+        return launch_band(T, K, st);
     }
-    if (!K.retry_only && T->has_stage && (o.kernel == DSP_KERNEL_AUTO || o.kernel == DSP_KERNEL_STAGE)) {
-        // generation-2 stage kernel: 32/L LPs per warp, persistent one-warp CTAs, LP groups refill from the ticket counter
-        const Stage2Geom g = stage2_geometry(T->sp.T);
-        const int per_warp = 32 / g.L;
-        // one persistent CTA per SM; its warps (up to kStage2Warps) run the phases of an IPM round in step
-        int wmax = kStage2Warps;
-        bool sync = true;
-        if (const char *e = getenv("DSP_STAGE2_WARPS")) wmax = std::min(kStage2Warps, std::max(1, atoi(e)));   // experiments only
-        if (const char *e = getenv("DSP_STAGE2_SYNC")) sync = atoi(e) != 0;
-        const long long warps_needed = (N + per_warp - 1) / per_warp;
-        const long long blocks = std::max<long long>(1, std::min<long long>(T->sm_count, warps_needed));
-        const int wpb = (int)std::min<long long>(wmax, (warps_needed + blocks - 1) / blocks);
-        const size_t smem = stage2_smem_bytes(g) * wpb;
-        stage2::Params Q;
-        Q.N = N; Q.cparams = cparams; Q.rparams = rparams; Q.rstride = rparams_stride; Q.Pc = K.Pc; Q.Pr = K.Pr;
-        Q.omap = K.omap; Q.ocmap = K.ocmap; Q.o0 = K.o0;
-        Q.tol = o.tol; Q.feas_tol = o.feas_tol; Q.step_frac = o.step_frac; Q.reg = o.reg_primal; Q.max_iter = o.max_iter;
-        Q.obj = obj; Q.x_out = x; Q.y_out = y; Q.status = status; Q.iters = iters; Q.n = K.n; Q.m = K.m; Q.ticket = ticket;
-        const stagewb::StageParams &S = T->sp;
-        Q.T = S.T; Q.a = S.a; Q.binv = S.binv; Q.hf = S.hf; Q.dl = S.dl; Q.dur = S.dur; Q.krev = S.krev;
-        Q.wcf_off = S.wcf_off; Q.p_off = S.p_off; Q.col_idx = S.col_idx; Q.row_idx = S.row_idx;
-        Q.ahead = (int)(blocks * wpb * per_warp);
-        CK(cudaMemsetAsync(ticket, 0, sizeof(unsigned long long), st));
-#define S2_LAUNCH(l, p)                                                                                      \
-        if (sync) dsp_ipm_stage2_wb_kernel<l, p, true><<<(unsigned)blocks, 32 * wpb, smem, st>>>(Q);             \
-        else dsp_ipm_stage2_wb_kernel<l, p, false><<<(unsigned)blocks, 32 * wpb, smem, st>>>(Q)
-        S2_DISPATCH(S2_LAUNCH);
-#undef S2_LAUNCH
-        CK(cudaGetLastError());
-        std::lock_guard<std::mutex> lk(g_mu);
-        g_launches++;
-        g_last_grid = (int)blocks; g_last_block = 32 * wpb; g_last_smem = (int)smem; g_last_ppc = per_warp * wpb;
-        return 0;
-    }
-    if (!K.retry_only && T->has_stage && o.kernel == DSP_KERNEL_STAGE_V1) {
-        if (T->sp.T > 32) { g_err = "dsp_lp_solve_batch: the lane-per-period stage kernel needs T <= 32"; return DSP_E_ARG; }
-        // generation-1 stage kernel (lane per period): no shared memory; persistent warps, one LP per warp at a time
-        const int wpb = DSP_STAGE_WPB;
-        long long per_sm = T->stage_blocks_per_sm;
-        if (const char *e = getenv("DSP_STAGE_BLOCKS_PER_SM")) per_sm = std::max(1, atoi(e));   // experiments only
-        long long blocks = std::min<long long>((long long)T->sm_count * per_sm, (N + wpb - 1) / wpb);
-        CK(cudaMemsetAsync(ticket, 0, sizeof(unsigned long long), st));
-        dsp_ipm_stage_wb_kernel<<<(unsigned)blocks, wpb * 32, 0, st>>>(K, T->sp);
-        CK(cudaGetLastError());
-        std::lock_guard<std::mutex> lk(g_mu);
-        g_launches++;
-        g_last_grid = (int)blocks; g_last_block = wpb * 32; g_last_smem = 0; g_last_ppc = wpb;
-        return 0;
-    }
-    if (!K.retry_only && T->has_chain1 && (o.kernel == DSP_KERNEL_AUTO || o.kernel == DSP_KERNEL_STAGE)) {
-        const int L = chain1_lanes(T->c1_T), per_warp = 32 / L, NF = T->c1_NF;
-        int wmax = chain1_warps(NF);
-        if (const char *e = getenv("DSP_CHAIN1_WARPS")) wmax = std::min(wmax, std::max(1, atoi(e)));      // experiments only
-        const long long warps_needed = (N + per_warp - 1) / per_warp;
-        const long long blocks = std::max<long long>(1, std::min<long long>(T->sm_count, warps_needed));
-        const int wpb = (int)std::min<long long>(wmax, (warps_needed + blocks - 1) / blocks);
-        const size_t smem = (size_t)(NF == 2 ? chain1::Smem<2, 3>::doubles_per_warp : chain1::Smem<3, 3>::doubles_per_warp) * 8 * wpb;
-        chain1::Params Q;
-        Q.N = N; Q.cparams = cparams; Q.rparams = rparams; Q.rstride = rparams_stride; Q.Pc = K.Pc; Q.Pr = K.Pr;
-        Q.omap = K.omap; Q.ocmap = K.ocmap; Q.o0 = K.o0;
-        Q.tol = o.tol; Q.feas_tol = o.feas_tol; Q.step_frac = o.step_frac; Q.reg = o.reg_primal; Q.max_iter = o.max_iter;
-        Q.obj = obj; Q.x_out = x; Q.y_out = y; Q.status = status; Q.iters = iters; Q.n = K.n; Q.m = K.m; Q.nb = K.nb; Q.ticket = ticket;
-        Q.c0 = K.c0; Q.b0 = K.b0; Q.u0 = K.u0; Q.cm_ptr = K.cm_ptr; Q.cm_idx = K.cm_idx; Q.cm_val = K.cm_val;
-        Q.bm_ptr = K.bm_ptr; Q.bm_idx = K.bm_idx; Q.bm_val = K.bm_val; Q.um_ptr = K.um_ptr; Q.um_idx = K.um_idx; Q.um_val = K.um_val;
-        Q.T = T->c1_T; Q.col_idx = T->c1_col_idx; Q.row_idx = T->c1_row_idx; Q.coef = T->c1_coef; Q.coef_next = T->c1_coef_next;
-        Q.x_perm = K.xperm; Q.y_perm = K.yperm;
-        CK(cudaMemsetAsync(ticket, 0, sizeof(unsigned long long), st));
-#define C1_LAUNCH(l, nf) dsp_ipm_stage_chain1_kernel<l, 3, nf><<<(unsigned)blocks, 32 * wpb, smem, st>>>(Q)
-        if (NF == 2) { if (L == 4) C1_LAUNCH(4, 2); else if (L == 8) C1_LAUNCH(8, 2); else if (L == 16) C1_LAUNCH(16, 2); else C1_LAUNCH(32, 2); }
-        else { if (L == 4) C1_LAUNCH(4, 3); else if (L == 8) C1_LAUNCH(8, 3); else if (L == 16) C1_LAUNCH(16, 3); else C1_LAUNCH(32, 3); }
-#undef C1_LAUNCH
-        CK(cudaGetLastError());
-        std::lock_guard<std::mutex> lk(g_mu);
-        g_launches++;
-        g_last_grid = (int)blocks; g_last_block = 32 * wpb; g_last_smem = (int)smem; g_last_ppc = per_warp * wpb;
-        return 0;
-    }
-    if (!K.retry_only && (o.kernel == DSP_KERNEL_STAGE || o.kernel == DSP_KERNEL_STAGE_V1)) {
+    if (T->has_stage && stage) return launch_stage2(T, K, st);
+    if (T->has_stage && o.kernel == DSP_KERNEL_STAGE_V1) return launch_stage_v1(T, K, st);
+    if (T->has_chain1 && stage) return launch_chain1(T, K, st);
+    if (o.kernel == DSP_KERNEL_STAGE || o.kernel == DSP_KERNEL_STAGE_V1) {
         g_err = "dsp_lp_solve_batch: the template has no stage descriptor";
         return DSP_E_ARG;
     }
-    const size_t prob_bytes = (size_t)K.prob_doubles * 8;
-    const BandGeom geom = band_geometry(T, K);
-#ifdef DSP_EXPERIMENT_HYBRID2
-    if (geom.hybrid == 2) K.band_doubles += 2 * K.n;
-#endif
-    const size_t band_bytes = (size_t)K.band_doubles * 8;
-    long long warps = geom.warps;
-    const int hot_in_smem = geom.hot_in_smem, hybrid = geom.hybrid;
-    const size_t off = geom.off;
-    const bool ws_mode = geom.ws;
-    long long ctas = std::min<long long>(T->sm_count, (N + warps - 1) / warps);
-    // spread a small batch over all SMs
-    if (ctas < T->sm_count && N > ctas) {
-        ctas = std::min<long long>(T->sm_count, N);
-        warps = std::min<long long>(warps, (N + ctas - 1) / ctas);
-    }
-    K.hot_in_smem = hot_in_smem;
-    K.prob_off = (int)off;
-    K.ws = nullptr;
-    size_t smem = off + (size_t)warps * prob_bytes;
-    if (ws_mode) {
-        const size_t need = (size_t)ctas * (size_t)warps * prob_bytes;
-        if (need > T->ws_bytes) {
-            CK(cudaStreamSynchronize(st));
-            cudaFree(T->ws);
-            T->ws = nullptr; T->ws_bytes = 0;
-            CK(cudaMalloc((void **)&T->ws, need));
-            T->ws_bytes = need;
-        }
-        K.ws = T->ws;
-        smem = hybrid ? off + (size_t)warps * band_bytes : 16;
-    }
-    K.hybrid = hybrid;
-    CK(cudaMemsetAsync(ticket, 0, sizeof(unsigned long long), st));
-    switch (K.w) {
-        case 1: if (ws_mode) dsp_ipm_band_kernel<1, true, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                else if (hot_in_smem) dsp_ipm_band_kernel<1, false, true><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                else dsp_ipm_band_kernel<1, false, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                break;
-        case 2: if (ws_mode) dsp_ipm_band_kernel<2, true, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                else if (hot_in_smem) dsp_ipm_band_kernel<2, false, true><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                else dsp_ipm_band_kernel<2, false, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                break;
-        case 4: if (ws_mode) dsp_ipm_band_kernel<4, true, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                else if (hot_in_smem) dsp_ipm_band_kernel<4, false, true><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                else dsp_ipm_band_kernel<4, false, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                break;
-        case 8: if (ws_mode) dsp_ipm_band_kernel<8, true, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                else if (hot_in_smem) dsp_ipm_band_kernel<8, false, true><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                else dsp_ipm_band_kernel<8, false, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                break;
-        case 16: if (ws_mode) dsp_ipm_band_kernel<16, true, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                 else if (hot_in_smem) dsp_ipm_band_kernel<16, false, true><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                 else dsp_ipm_band_kernel<16, false, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                 break;
-        default: if (ws_mode) dsp_ipm_band_kernel<32, true, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                 else if (hot_in_smem) dsp_ipm_band_kernel<32, false, true><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                 else dsp_ipm_band_kernel<32, false, false><<<(unsigned)ctas, (unsigned)(warps * 32), smem, st>>>(K);
-                 break;
-    }
-    CK(cudaGetLastError());
-    {
-        std::lock_guard<std::mutex> lk(g_mu);
-        g_launches++;
-        g_last_grid = (int)ctas; g_last_block = (int)(warps * 32); g_last_smem = (int)smem; g_last_ppc = (int)warps;
-    }
-    return 0;
+    return launch_band(T, K, st);
 }
 
 int dsp_lp_solve_batch(const dsp_template *T, int64_t N, const double *cparams, const double *rparams,

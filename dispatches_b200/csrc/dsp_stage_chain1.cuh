@@ -71,7 +71,9 @@ struct Per {
     double y;
 };
 
-template <int L, int P, int NF, bool CTA_SYNC>
+// The trailing flag is ignored: the exit vote is always the CTA barrier on the device and the warp vote in the emulator
+// (stage2::cta_all).  tests/emu/emu_chain1.cpp still passes it, so it stays in the signature.
+template <int L, int P, int NF, bool = true>
 __device__ void warp_body(const Params &Q, double *smw, int lane) {
     using SM = Smem<NF, P>;
     constexpr int NC = NF + 1;
@@ -338,7 +340,7 @@ __device__ void warp_body(const Params &Q, double *smw, int lane) {
             mu0 = gsum<L>(mu0);
             if (ld) mu_keep = mu0 / ntot;      // (the start point is never optimal: its own convergence check is skipped)
         }
-        if (cta_all<CTA_SYNC>(mode == 3)) break;
+        if (cta_all(mode == 3)) break;
         if (__all_sync(FULL, mode == 3)) continue;     // out of work: leave the issue slots to the warps that still iterate
 
         // =========================================================================================== neighbours of the lane's block

@@ -71,26 +71,6 @@ __device__ __forceinline__ double wsum(double v) {
     return v;
 }
 
-#ifdef DSP_STAGE_PARK
-// round-2 experiment (tools/build_variants.py): values that are computed early in an iteration and reused by the predictor
-// AND the corrector are parked in shared memory (22 doubles per lane) so that the kernel fits 128 registers / 16 warps per SM
-#define PARK_ST(k, v) park[(k) * 32] = (v)
-#define PARK_LD(k, v) park[(k) * 32]
-#define PARK_PARAM , double *park
-#if DSP_STAGE_PARK >= 2      // also the right-hand-side pieces that wait for the solves and the predictor's second-order products
-#define PARK2_ST(k, v) park[(k) * 32] = (v)
-#define PARK2_LD(k, v) park[(k) * 32]
-#endif
-#else
-#define PARK_ST(k, v) ((void)0)
-#define PARK_LD(k, v) (v)
-#define PARK_PARAM
-#endif
-#ifndef PARK2_ST
-#define PARK2_ST(k, v) ((void)0)
-#define PARK2_LD(k, v) (v)
-#endif
-
 struct Sym2 { double a, b, c; };            // [[a, b], [b, c]]
 struct Mat2 { double a, b, c, d; };         // [[a, b], [c, d]]
 
@@ -177,7 +157,7 @@ struct Out {
 // is a run-time value: the iteration body is ~3k instructions, and a T=24 instantiation with unrolled sweeps (7k) ran
 // slower, limited by instruction-cache misses
 __device__ int solve_one(const StageParams &S, const double *cp, const double *rpar, double kconst, long long p,
-                          double tol, double feas_tol, double step_frac, double reg, int max_iter, const Out &O, int lane, int it0 PARK_PARAM) {
+                          double tol, double feas_tol, double step_frac, double reg, int max_iter, const Out &O, int lane, int it0) {
     const int T = S.T;
     const bool act = lane < T, has_s = lane < T - 1;
     const double a = S.a, binv = S.binv, hf = S.hf, dl = S.dl;
@@ -204,22 +184,6 @@ __device__ int solve_one(const StageParams &S, const double *cp, const double *r
     double xg = 1.0, xi = fmin(1.0, 0.5 * u), xo = xi, xs = has_s ? 1.0 : 0.0, xe = 1.0, xp = 1.0, xq = 1.0;
     double zg = 1.0, zi = 1.0, zo = 1.0, zs = has_s ? 1.0 : 0.0, ze = 1.0, zp = 1.0, zq = 1.0;
     double si = u - xi, so = u - xo, wi = 1.0, wo = 1.0;
-#if defined(DSP_STAGE_START) && DSP_STAGE_START == 1
-    // round-2 experiment (oracle/ipm_stage_numpy.py start_mode=1): a primal start that satisfies the wind-balance and
-    // SoC-bound rows exactly; 11.38 vs 11.80 iterations on C2, 10.7 vs 12.5 on C5 in the mirror (with step_frac 0.99995)
-    {
-        xg = dmax(0.5 * b4, 1e-2);
-        xi = fmin(fmin(1.0, 0.5 * u), dmax(0.25 * b4, 1e-2)); xo = xi;
-        xq = dmax(b4 - xg - xi, 1e-2);
-        xs = has_s ? dmax(0.5 * b3, 1e-2) : 0.0;
-        double cum = act ? xi + xo : 0.0;                      // inclusive prefix sum over the periods
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const double v = __shfl_up_sync(0xffffffffu, cum, o); if (lane >= o) cum += v; }
-        xe = dmax(0.5 * cum, 1e-2);
-        xp = dmax(b3 - xs - dl * xe, 1e-2);
-        si = u - xi; so = u - xo;
-    }
-#endif
     double y1 = 0.0, y2 = 0.0, y3 = 0.0, y4 = 0.0;
     // ---- twisted elimination order
     Factor F;
@@ -273,7 +237,6 @@ __device__ int solve_one(const StageParams &S, const double *cp, const double *r
             break;
         }
         if (it == max_iter) break;
-        PARK_ST(0, rp1); PARK_ST(1, rp2); PARK_ST(2, rp3); PARK_ST(3, rp4); PARK_ST(4, rdg); PARK_ST(5, rdi); PARK_ST(6, rdo); PARK_ST(7, rds); PARK_ST(8, rde); PARK_ST(9, rdp); PARK_ST(10, rdq); PARK_ST(11, rui); PARK_ST(12, ruo);
         PH(8);
         // ---- scaling matrix D and reciprocals
         const double rxg = frcp(xg), rxi = frcp(xi), rxo = frcp(xo), rxe = frcp(xe), rxp = frcp(xp), rxq = frcp(xq);
@@ -281,7 +244,6 @@ __device__ int solve_one(const StageParams &S, const double *cp, const double *r
         const double rsi = frcp(si), rso = frcp(so);
         const double rzg = frcp(zg), rze = frcp(ze), rzp = frcp(zp), rzq = frcp(zq), rzs = has_s ? frcp(zs) : 0.0;
         const double rzi = frcp(zi), rzo = frcp(zo), rwi = frcp(wi), rwo = frcp(wo);
-        PARK_ST(13, rzg); PARK_ST(14, rzi); PARK_ST(15, rzo); PARK_ST(16, rzs); PARK_ST(17, rze); PARK_ST(18, rzp); PARK_ST(19, rzq); PARK_ST(20, rwi); PARK_ST(21, rwo);
         // d = 1 / (z/x [+ w/s] + reg / max(1, x^2)): the proximal term caps d for columns that never approach a bound;
         // dividing by x^2 for x > 1 keeps it scale invariant (the throughput column grows with the horizon)
         const double qg = xg > 1.0 ? reg * rxg * rxg : reg, qe = xe > 1.0 ? reg * rxe * rxe : reg;
@@ -316,39 +278,38 @@ __device__ int solve_one(const StageParams &S, const double *cp, const double *r
         double smu = 0.0;
         double hg, hi, ho, hs, he, hp, hq, w3, w4;
         auto make_rhs = [&](bool corr, double &f1, double &f2) {
-            hg = PARK_LD(4, rdg) + zg; hi = PARK_LD(5, rdi) + zi; ho = PARK_LD(6, rdo) + zo; hs = PARK_LD(7, rds) + zs; he = PARK_LD(8, rde) + ze; hp = PARK_LD(9, rdp) + zp; hq = PARK_LD(10, rdq) + zq;
-            double asi = -wi * PARK_LD(11, rui), aso = -wo * PARK_LD(12, ruo);
+            hg = rdg + zg; hi = rdi + zi; ho = rdo + zo; hs = rds + zs; he = rde + ze; hp = rdp + zp; hq = rdq + zq;
+            double asi = -wi * rui, aso = -wo * ruo;
             if (corr) {
-                hg -= (smu - PARK2_LD(31, cg)) * rxg; hi -= (smu - PARK2_LD(32, ci)) * rxi; ho -= (smu - PARK2_LD(33, co)) * rxo; hs -= (smu - PARK2_LD(34, cs)) * rxs;
-                he -= (smu - PARK2_LD(35, ce)) * rxe; hp -= (smu - PARK2_LD(36, cpp)) * rxp; hq -= (smu - PARK2_LD(37, cq)) * rxq;
-                asi += smu - PARK2_LD(38, csi); aso += smu - PARK2_LD(39, cso);
+                hg -= (smu - cg) * rxg; hi -= (smu - ci) * rxi; ho -= (smu - co) * rxo; hs -= (smu - cs) * rxs;
+                he -= (smu - ce) * rxe; hp -= (smu - cpp) * rxp; hq -= (smu - cq) * rxq;
+                asi += smu - csi; aso += smu - cso;
             }
             hi += asi * rsi - wi; ho += aso * rso - wo;
             if (!has_s) hs = 0.0;
-            w3 = PARK_LD(2, rp3) + dp * hp;
+            w3 = rp3 + dp * hp;
             const double ph1 = s11 * hs - s12 * he - dsk * w3;
             const double ph2 = s22 * he - s12 * hs - dek * w3;
-            w4 = PARK_LD(3, rp4) + dg * hg + dq * hq;
+            w4 = rp4 + dg * hg + dq * hq;
             const double psi = tau * hi - dii * w4;
             const double doh = dO * ho;
-            f1 = PARK_LD(0, rp1) + ph1 - up1(ph1, lane) - a * psi + binv * doh;
-            f2 = PARK_LD(1, rp2) + ph2 - up1(ph2, lane) - hf * psi - hf * doh;
+            f1 = rp1 + ph1 - up1(ph1, lane) - a * psi + binv * doh;
+            f2 = rp2 + ph2 - up1(ph2, lane) - hf * psi - hf * doh;
             if (!act) { f1 = 0.0; f2 = 0.0; }
-            PARK2_ST(22, hg); PARK2_ST(23, hi); PARK2_ST(24, ho); PARK2_ST(25, hs); PARK2_ST(26, he); PARK2_ST(27, hp); PARK2_ST(28, hq); PARK2_ST(29, w3); PARK2_ST(30, w4);
         };
         auto recover = [&](double u1, double u2) {
             dy1 = u1; dy2 = u2;
-            const double e1 = dy1 - down1(dy1, lane) - PARK2_LD(25, hs), e2 = dy2 - down1(dy2, lane) - PARK2_LD(26, he);
+            const double e1 = dy1 - down1(dy1, lane) - hs, e2 = dy2 - down1(dy2, lane) - he;
             const double v = a * dy1 + hf * dy2;
-            dxs = has_s ? s11 * e1 - s12 * e2 + dsk * PARK2_LD(29, w3) : 0.0;
-            dxe = s22 * e2 - s12 * e1 + dek * PARK2_LD(29, w3);
-            dxi = -tau * (v + PARK2_LD(23, hi)) + dii * PARK2_LD(30, w4);
-            dxo = dO * (binv * dy1 - hf * dy2 - PARK2_LD(24, ho));
-            dxg = dg * iot * (PARK_LD(3, rp4) + di * (PARK2_LD(23, hi) - PARK2_LD(22, hg) + v) + dq * (PARK2_LD(28, hq) - PARK2_LD(22, hg)));
-            dy3 = kap * (PARK2_LD(29, w3) - ds * e1 - dl * de * e2);
-            dy4 = iot * (PARK2_LD(30, w4) + di * (PARK2_LD(23, hi) + v));
-            dxp = dp * (dy3 - PARK2_LD(27, hp));
-            dxq = dq * (dy4 - PARK2_LD(28, hq));
+            dxs = has_s ? s11 * e1 - s12 * e2 + dsk * w3 : 0.0;
+            dxe = s22 * e2 - s12 * e1 + dek * w3;
+            dxi = -tau * (v + hi) + dii * w4;
+            dxo = dO * (binv * dy1 - hf * dy2 - ho);
+            dxg = dg * iot * (rp4 + di * (hi - hg + v) + dq * (hq - hg));
+            dy3 = kap * (w3 - ds * e1 - dl * de * e2);
+            dy4 = iot * (w4 + di * (hi + v));
+            dxp = dp * (dy3 - hp);
+            dxq = dq * (dy4 - hq);
         };
         // ---- twisted block LDL'; the forward elimination of the PREDICTOR right-hand side rides along in the same
         // ---- sweep (its shuffles and FMAs fill the latency shadow of the 2x2 inversions)
@@ -404,14 +365,14 @@ __device__ int solve_one(const StageParams &S, const double *cp, const double *r
         double dzg = -zg - zg * dxg * rxg, dzi = -zi - zi * dxi * rxi, dzo = -zo - zo * dxo * rxo;
         double dzs = has_s ? -zs - zs * dxs * rxs : 0.0, dze = -ze - ze * dxe * rxe, dzp = -zp - zp * dxp * rxp;
         double dzq = -zq - zq * dxq * rxq;
-        double dsi = PARK_LD(11, rui) - dxi, dso = PARK_LD(12, ruo) - dxo;
+        double dsi = rui - dxi, dso = ruo - dxo;
         double dwi = -wi - wi * dsi * rsi, dwo = -wo - wo * dso * rso;
         double ip = 0.0, id = 0.0;             // 1/alpha
         if (act) {
             ip = dmax(dmax(dmax(-dxg * rxg, -dxi * rxi), dmax(-dxo * rxo, -dxs * rxs)), dmax(dmax(-dxe * rxe, -dxp * rxp), -dxq * rxq));
             ip = dmax(ip, dmax(-dsi * rsi, -dso * rso));
-            id = dmax(dmax(dmax(-dzg * PARK_LD(13, rzg), -dzi * PARK_LD(14, rzi)), dmax(-dzo * PARK_LD(15, rzo), -dzs * PARK_LD(16, rzs))), dmax(dmax(-dze * PARK_LD(17, rze), -dzp * PARK_LD(18, rzp)), -dzq * PARK_LD(19, rzq)));
-            id = dmax(id, dmax(-dwi * PARK_LD(20, rwi), -dwo * PARK_LD(21, rwo)));
+            id = dmax(dmax(dmax(-dzg * rzg, -dzi * rzi), dmax(-dzo * rzo, -dzs * rzs)), dmax(dmax(-dze * rze, -dzp * rzp), -dzq * rzq));
+            id = dmax(id, dmax(-dwi * rwi, -dwo * rwo));
         }
         ip = wmax_pos(ip); id = wmax_pos(id);
         double ap = ip > 1.0 ? 1.0 / ip : 1.0, ad = id > 1.0 ? 1.0 / id : 1.0;
@@ -424,7 +385,6 @@ __device__ int solve_one(const StageParams &S, const double *cp, const double *r
         mua = wsum(mua) / ntot;
         cg = dxg * dzg; ci = dxi * dzi; co = dxo * dzo; cs = dxs * dzs; ce = dxe * dze; cpp = dxp * dzp; cq = dxq * dzq;
         csi = dsi * dwi; cso = dso * dwo;
-        PARK2_ST(31, cg); PARK2_ST(32, ci); PARK2_ST(33, co); PARK2_ST(34, cs); PARK2_ST(35, ce); PARK2_ST(36, cpp); PARK2_ST(37, cq); PARK2_ST(38, csi); PARK2_ST(39, cso);
         const double sg = mua / mu;
         smu = sg * sg * sg * mu;
         PH(13);
@@ -433,18 +393,18 @@ __device__ int solve_one(const StageParams &S, const double *cp, const double *r
         tw_solve(F, g1, g2, T, lane);
         PH(14);
         recover(g1, g2);
-        dzg = (smu - PARK2_LD(31, cg)) * rxg - zg - zg * dxg * rxg; dzi = (smu - PARK2_LD(32, ci)) * rxi - zi - zi * dxi * rxi;
-        dzo = (smu - PARK2_LD(33, co)) * rxo - zo - zo * dxo * rxo; dzs = has_s ? (smu - PARK2_LD(34, cs)) * rxs - zs - zs * dxs * rxs : 0.0;
-        dze = (smu - PARK2_LD(35, ce)) * rxe - ze - ze * dxe * rxe; dzp = (smu - PARK2_LD(36, cpp)) * rxp - zp - zp * dxp * rxp;
-        dzq = (smu - PARK2_LD(37, cq)) * rxq - zq - zq * dxq * rxq;
-        dsi = PARK_LD(11, rui) - dxi; dso = PARK_LD(12, ruo) - dxo;
-        dwi = (smu - PARK2_LD(38, csi)) * rsi - wi - wi * dsi * rsi; dwo = (smu - PARK2_LD(39, cso)) * rso - wo - wo * dso * rso;
+        dzg = (smu - cg) * rxg - zg - zg * dxg * rxg; dzi = (smu - ci) * rxi - zi - zi * dxi * rxi;
+        dzo = (smu - co) * rxo - zo - zo * dxo * rxo; dzs = has_s ? (smu - cs) * rxs - zs - zs * dxs * rxs : 0.0;
+        dze = (smu - ce) * rxe - ze - ze * dxe * rxe; dzp = (smu - cpp) * rxp - zp - zp * dxp * rxp;
+        dzq = (smu - cq) * rxq - zq - zq * dxq * rxq;
+        dsi = rui - dxi; dso = ruo - dxo;
+        dwi = (smu - csi) * rsi - wi - wi * dsi * rsi; dwo = (smu - cso) * rso - wo - wo * dso * rso;
         ip = 0.0; id = 0.0;
         if (act) {
             ip = dmax(dmax(dmax(-dxg * rxg, -dxi * rxi), dmax(-dxo * rxo, -dxs * rxs)), dmax(dmax(-dxe * rxe, -dxp * rxp), -dxq * rxq));
             ip = dmax(ip, dmax(-dsi * rsi, -dso * rso));
-            id = dmax(dmax(dmax(-dzg * PARK_LD(13, rzg), -dzi * PARK_LD(14, rzi)), dmax(-dzo * PARK_LD(15, rzo), -dzs * PARK_LD(16, rzs))), dmax(dmax(-dze * PARK_LD(17, rze), -dzp * PARK_LD(18, rzp)), -dzq * PARK_LD(19, rzq)));
-            id = dmax(id, dmax(-dwi * PARK_LD(20, rwi), -dwo * PARK_LD(21, rwo)));
+            id = dmax(dmax(dmax(-dzg * rzg, -dzi * rzi), dmax(-dzo * rzo, -dzs * rzs)), dmax(dmax(-dze * rze, -dzp * rzp), -dzq * rzq));
+            id = dmax(id, dmax(-dwi * rwi, -dwo * rwo));
         }
         ip = wmax_pos(ip); id = wmax_pos(id);
         ap = (step_frac * 1.0 < ip) ? step_frac / ip : 1.0;     // min(1, step_frac / ip)

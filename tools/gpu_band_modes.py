@@ -1,8 +1,15 @@
-"""band kernel: the three placements of the per-LP work region (env DSP_BAND_MODE = smem | hybrid | ws) across templates"""
+"""band kernel: the three placements of the per-LP work region (env DSP_BAND_MODE = smem | hybrid | ws) across templates
+
+needs a -DDSP_PHASES build of the library, named by DSP_LP_LIB (see tools/gpu_stage2_phases.py): the product library reads no
+environment, so only the instrumentation build takes DSP_BAND_MODE.  The placements are therefore compared with the phase
+counters compiled in.
+"""
 import sys, os, json
 sys.path.insert(0, ".")
 import numpy as np, torch
 from dispatches_b200 import templates as TP, scenarios as SC, solver as S
+if not hasattr(S.load_library(), "dsp_lp_phases"):
+    raise SystemExit(f"{S._LIB_PATH} is not a -DDSP_PHASES build: it ignores DSP_BAND_MODE")
 dev = torch.device("cuda:0")
 rng = np.random.default_rng(3)
 cases = {}
@@ -23,7 +30,7 @@ cases["wind_battery_pem_T24"] = (TP.wind_battery_pem(24), torch.tensor(np.concat
                                  torch.tensor(TP.wind_battery_rparams(24, cf2, W2, 150.0, pem_mw=200.0)[0], device=dev))
 cases["C3_nuclear_T48"] = (TP.nuclear(48), torch.tensor(SC.c3(5000), device=dev), None)
 MODES = [a.split("=")[1] for a in sys.argv if a.startswith("--modes=")]
-MODES = MODES[0].split(",") if MODES else ["smem", "hybrid", "ws"]      # hybrid2 needs a -DDSP_EXPERIMENT_HYBRID2 build (DSP_LP_LIB)
+MODES = MODES[0].split(",") if MODES else ["smem", "hybrid", "ws"]
 out = {}
 for name, (t, cp, rp) in cases.items():
     sol = S.BatchLPSolver(t)

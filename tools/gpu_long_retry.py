@@ -1,6 +1,6 @@
-"""the full-year design sweep (64 LPs, T = 8736) on the AUTO path: long stage kernel + the band kernel's retry pass over the LPs it
-left non-optimal; DSP_LONG_NO_RETRY=1 (kernel STAGE) shows the long kernel alone"""
-import sys, os, json
+"""the full-year design sweep (64 LPs, T = 8736) on the stage path: long stage kernel + the band kernel's retry pass over the LPs it
+left non-optimal"""
+import sys
 sys.path.insert(0, ".")
 import numpy as np, torch
 from dispatches_b200 import templates as TP, scenarios as SC, solver as S
@@ -19,5 +19,5 @@ o = sol.solve(cpd, rpd); torch.cuda.synchronize()
 e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
 e0.record(); o = sol.solve(cpd, rpd, out=o); e1.record(); torch.cuda.synchronize()
 st = o.status.cpu().numpy()
-print("retry" if not os.environ.get("DSP_LONG_NO_RETRY") else "long kernel alone", "%.1f ms" % e0.elapsed_time(e1), "non-optimal", np.nonzero(st)[0].tolist(),
+print("%.1f ms" % e0.elapsed_time(e1), "non-optimal", np.nonzero(st)[0].tolist(),
       "iters", o.iters.cpu().numpy().tolist(), "obj[19] %.10e" % float(o.obj[19]), flush=True)

@@ -1,5 +1,5 @@
 """stage kernel generation 2 vs generation 1 vs band kernel: parity + timing on C2 (10 000 LPs) and a C5 slice; other horizons."""
-import sys, os, json, time
+import sys, json
 sys.path.insert(0, ".")
 import numpy as np, torch
 from dispatches_b200 import templates as TP, scenarios as SC, solver as S
@@ -27,12 +27,6 @@ out["C2"] = dict(v2_ms=ms2, v2_min_ms=mn2, v1_ms=ms1, v1_min_ms=mn1, speedup=ms1
                  v2_non_optimal=int((a.status != 0).sum()), iters_v2=float(a.iters.float().mean()), iters_v1=float(b.iters.float().mean()),
                  iters_equal=float((a.iters == b.iters).float().mean()), rel_v2_v1=rel(ao, bo), rel_v2_band=rel(ao[:1024], co))
 print(json.dumps(out["C2"]), flush=True)
-for bps in (4, 5, 6, 7, 8):
-    os.environ["DSP_STAGE2_BLOCKS_PER_SM"] = str(bps)
-    _, ms, mn = timed(v2, cp, rpt, reps=5)
-    out[f"C2_blocks_per_sm_{bps}"] = dict(ms=ms, min_ms=mn, launch=S.last_launch())
-    print(bps, ms, mn, S.last_launch(), flush=True)
-del os.environ["DSP_STAGE2_BLOCKS_PER_SM"]
 # x / y write-back parity
 ax = v2.solve(cp[:2048], rpt, want_x=True, want_y=True); bx = v1.solve(cp[:2048], rpt, want_x=True, want_y=True); torch.cuda.synchronize()
 out["xy"] = dict(x_maxdiff=float((ax.x - bx.x).abs().max()), y_maxdiff=float((ax.y - bx.y).abs().max()), x_scale=float(bx.x.abs().max()), y_scale=float(bx.y.abs().max()))

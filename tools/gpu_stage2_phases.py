@@ -3,7 +3,9 @@
 needs a -DDSP_PHASES build of the library, named by DSP_LP_LIB:
     nvcc <NVCC_FLAGS of dispatches_b200/csrc/build.py> -DDSP_PHASES dispatches_b200/csrc/dsp_lp.cu -o build/phases/libdsp_lp.so
     DSP_LP_LIB=$PWD/build/phases/libdsp_lp.so python tools/gpu_stage2_phases.py [warps ...]
-The counters (dsp_stage2.cuh) sum over warp 0 of every CTA; 8 warps per SM are two per scheduler, 4 are one.
+The counters (dsp_stage2.cuh) sum over warp 0 of every CTA; 8 warps per SM are two per scheduler, 4 are one.  Only this
+instrumentation build reads DSP_STAGE2_WARPS (the product library reads no environment), so the 8- vs 4-warp comparison runs
+with the counters compiled in.
 """
 import ctypes as C
 import os
