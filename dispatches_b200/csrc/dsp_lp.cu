@@ -29,6 +29,7 @@
 #include <vector>
 
 #include "dsp_band.cuh"
+#include "dsp_nan_rows.cuh"
 
 #define DSP_VERSION "dsp_lp 0.2 (sm_90a band-IPM + stage kernels)"
 
@@ -298,6 +299,7 @@ __device__ void solve_one(const Work &W, const Hot &H0, const KParams &P, long l
     __syncwarp();
     if (__any_sync(0xffffffffu, bad_u)) {
         if (lane == 0) { P.obj[p] = __longlong_as_double(0x7ff8000000000000LL); P.status[p] = DSP_INFEASIBLE; P.iters[p] = it0; }
+        dsp_nan_rows(P.x_out, n, P.y_out, m, p, lane, 32);
         *status_out = DSP_OPTIMAL;          // no second attempt
         *iters_out = it0;
         return;

@@ -94,13 +94,14 @@ __device__ int solve_long(const LongParams &LQ, double *wsw, long long p, int la
     }
     kc = gsum<L>(kc); b4m = gmax<L>(b4m); cm = gmax<L>(cm);
     const double kconst = kc + Q.o0;
-    if (Pw < 0.0) {
-        if (lane == 0) { Q.obj[p] = __longlong_as_double(0x7ff8000000000000LL); Q.status[p] = DSP_INFEASIBLE; Q.iters[p] = it0; }
-        return 0;
-    }
     const double b3u = Q.dur * Pw;
     double beta_b = dmax(dmax(fabs(b3u), b4m), Pw);
     beta_b = beta_b > 0.0 ? beta_b : 1.0;
+    if (Pw < -1e-9 * beta_b) {      // negative battery power bound beyond rounding: infeasible (the band kernel's rule)
+        if (lane == 0) { Q.obj[p] = __longlong_as_double(0x7ff8000000000000LL); Q.status[p] = DSP_INFEASIBLE; Q.iters[p] = it0; }
+        dsp_nan_rows(Q.x_out, Q.n, Q.y_out, Q.m, p, lane, 32);
+        return 0;
+    }
     const double beta_c = cm > 0.0 ? cm : 1.0;
     const double b3 = b3u / beta_b, u = dmax(Pw / beta_b, 1e-10);
     const double nrm_b = 1.0 + dmax(fabs(b3), b4m / beta_b), nrm_c = 1.0 + (cm > 0.0 ? 1.0 : 0.0);

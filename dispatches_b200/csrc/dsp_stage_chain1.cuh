@@ -298,6 +298,7 @@ __device__ void warp_body(const Params &Q, double *smw, int lane) {
             if (ld) {
                 if (infl > 0.0) {
                     if (gl == 0) { Q.obj[p] = __longlong_as_double(0x7ff8000000000000LL); Q.status[p] = DSP_INFEASIBLE; Q.iters[p] = it0; }
+                    dsp_nan_rows(Q.x_out, Q.n, Q.y_out, Q.m, p, gl, L);
                     mode = 1; Tg = 0;
 #pragma unroll
                     for (int j = 0; j < P; ++j) {           // (an all-inactive group must not carry the finished LP's iterate)

@@ -17,6 +17,7 @@
 //   * Mehrotra predictor-corrector, same scaling / start / stopping rules as the generic kernel.
 // HBM traffic per LP: 8T (LMP row) in, 16 B out (+ x, y on request).  FP64 throughout.
 #pragma once
+#include "dsp_nan_rows.cuh"
 
 namespace stagewb {
 
@@ -165,15 +166,16 @@ __device__ int solve_one(const StageParams &S, const double *cp, const double *r
     const double lam = act ? cp[lane] : 0.0;
     const double wcf = act ? rpar[S.wcf_off + lane] : 0.0;
     const double P = rpar[S.p_off];
-    if (P < 0.0) {                  // negative battery power bound: infeasible (not silently clamped)
-        if (lane == 0) { O.obj[p] = __longlong_as_double(0x7ff8000000000000LL); O.status[p] = DSP_INFEASIBLE; O.iters[p] = it0; }
-        return 0;
-    }
     double c = S.krev * lam;
     double b3 = S.dur * P, b4 = wcf;
     const double b4max = wmax_pos(fabs(b4));
     double beta_b = dmax(dmax(fabs(b3), b4max), P);
     beta_b = beta_b > 0.0 ? beta_b : 1.0;
+    if (P < -1e-9 * beta_b) {       // negative battery power bound beyond rounding: infeasible (the band kernel's rule)
+        if (lane == 0) { O.obj[p] = __longlong_as_double(0x7ff8000000000000LL); O.status[p] = DSP_INFEASIBLE; O.iters[p] = it0; }
+        dsp_nan_rows(O.x_out, O.n, O.y_out, O.m, p, lane, 32);
+        return 0;
+    }
     const double cmax = wmax_pos(fabs(c));
     const double beta_c = cmax > 0.0 ? cmax : 1.0;
     c = c / beta_c; b3 = b3 / beta_b; b4 = b4 / beta_b;

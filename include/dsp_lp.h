@@ -114,7 +114,15 @@ int dsp_lp_template_set_stage_chain1(dsp_template *t, const dsp_stage_chain1_des
  * equations, residuals < 10 feas_tol and gap < 10 tol; OR complementarity < 1e-3 tol with residuals < 100 feas_tol and
  * gap < 1000 tol (the effective worst-case tolerance is therefore 1000 tol = 1e-6 relative on the LP part of the objective at
  * the defaults).  DSP_INFEASIBLE is reported only for a negative
- * upper bound produced by Umap / rparams (obj = NaN); other infeasible / unbounded LPs end as DSP_MAX_ITER / DSP_NUMERICAL. */
+ * upper bound produced by Umap / rparams; other infeasible / unbounded LPs end as DSP_MAX_ITER / DSP_NUMERICAL.  Every kernel
+ * applies one rule: u_j < -1e-9 * beta_b is infeasible, where beta_b = max(max_i |b_i|, max_j u_j) (1 if that is <= 0) is the
+ * LP's primal scale; a bound above that is clamped to 0 and the LP is solved (the 1e-9 is a rounding margin, far inside the 1e-7
+ * feasibility tolerance of CBC / HiGHS).  Only the bound is clamped: other data derived from the same parameter keep their value
+ * (the wind+battery state-of-charge right-hand side duration * P stays at its tiny negative value), so such an LP may still be
+ * infeasible by that rounding amount and end DSP_NUMERICAL / DSP_MAX_ITER, which of the two depending on the kernel.  An INFEASIBLE LP has obj = NaN, iters = iterations before the test (0 unless it is a retry), and,
+ * when x / y are requested, rows of NaN.
+ * iters counts the iterations of both attempts: an LP whose first attempt ends non-optimal is solved again (shorter step, stronger
+ * proximal term) and reports first + second, so with max_iter = k a non-optimal LP reports 2k.                              */
 enum { DSP_OPTIMAL = 0, DSP_MAX_ITER = 1, DSP_NUMERICAL = 2, DSP_INFEASIBLE = 3 };
 enum { DSP_E_ARG = -1, DSP_E_CUDA = -2, DSP_E_SMEM = -3, DSP_E_BUSY = -4 /* a host call is already in flight on this handle */ };
 

@@ -321,8 +321,8 @@ def test_stage_kernel_other_horizons(T):
 
 
 def test_design_opt_border_column():
-    """design_opt=True (battery size is a decision; per-period nameplate columns + link rows, half bandwidth > 8 so the
-    <16> instantiation of the band kernel): objective and optimal size against the oracle, through the reference API."""
+    """design_opt=True (battery size is a decision; per-period nameplate columns + link rows, half bandwidth 7, so the
+    <8> instantiation of the band kernel): objective and optimal size against the oracle, through the reference API."""
     lmp, cf, W, P = SC.c2(48)
     lmp[::3] *= 40.0                                 # scarcity days make a battery worth building
     t = TP.wind_battery_design(24)
