@@ -37,6 +37,7 @@ namespace {
 
 #ifdef DSP_PHASES            // developer instrumentation: per-phase cycle counters (warp 0 of block 0 accumulates)
 __device__ unsigned long long g_phase[16];
+__device__ int g_pass2_twice;    // stage 2 runs pass 2 of every round twice (DSP_STAGE2_PASS2_TWICE, tools/gpu_stage2_phases.py)
 #define PH_INIT long long ph_t0 = clock64();
 #define PH(k) do { long long ph_t1 = clock64(); if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&g_phase[k], (unsigned long long)(ph_t1 - ph_t0)); ph_t0 = clock64(); } while (0)
 #else
@@ -1080,6 +1081,11 @@ static int launch_stage2(const dsp_template *T, const KParams &K, cudaStream_t s
 #ifdef DSP_PHASES
     // instrumentation build only: tools/gpu_stage2_phases.py compares fewer warps per CTA (DSP_STAGE2_WARPS)
     if (const char *e = getenv("DSP_STAGE2_WARPS")) wmax = std::min(kStage2Warps, std::max(1, atoi(e)));
+    {   // ... and times a second copy of pass 2 in every round (DSP_STAGE2_PASS2_TWICE=1)
+        const char *e = getenv("DSP_STAGE2_PASS2_TWICE");
+        const int twice = e && atoi(e) ? 1 : 0;
+        CK(cudaMemcpyToSymbolAsync(g_pass2_twice, &twice, sizeof(int), 0, cudaMemcpyHostToDevice, st));
+    }
 #endif
     const long long warps_needed = (K.N + per_warp - 1) / per_warp;
     const long long blocks = std::max<long long>(1, std::min<long long>(T->sm_count, warps_needed));
