@@ -591,3 +591,44 @@ def detect_chain1(t: LPTemplate, max_flows=3):
         for f, j in enumerate(fl):
             col_idx[k, f] = j; coef[k, f] = Acsr[r, j]
     return dict(T=T, NF=int(NF), col_idx=col_idx, row_idx=np.array(order, np.int32), coef=coef, coef_next=coef_next)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+MAX_HALF_BANDWIDTH = 32              # widest band of A A' the band kernels are instantiated for
+MAX_LINKING_COLUMNS = 8
+
+
+def find_linking_columns(A, max_w=MAX_HALF_BANDWIDTH, max_k=MAX_LINKING_COLUMNS):
+    """Linking columns of a constraint matrix whose A A' is too wide for the band kernels: scalar columns (a design size, a capacity)
+    that sit in a row of every period.  Greedy: set aside the column with the most nonzeros, recompute the half bandwidth of the rest
+    (natural vs reverse Cuthill-McKee row order, as ``finalize``), and stop as soon as it is <= max_w.
+
+    Returns (cols, row_perm, w): the linking columns (sorted), the row order of the rest and its half bandwidth.  ``cols`` is empty
+    when A A' already fits (row_perm, w are then finalize's) or when more than max_k columns would be needed (w is then the full one)."""
+    A = abs(sp.csc_matrix(A))
+    m, n = A.shape
+
+    def order(keep):
+        P = (A[:, keep] @ A[:, keep].T).tocsr()
+        P.data[:] = 1.0
+        coo = P.tocoo()
+
+        def bw(perm):
+            inv = np.empty(m, int); inv[perm] = np.arange(m)
+            return int(np.max(np.abs(inv[coo.row] - inv[coo.col]))) if coo.nnz else 0
+        nat = np.arange(m)
+        rcm = np.asarray(reverse_cuthill_mckee(P, symmetric_mode=True))
+        return (nat, bw(nat)) if bw(nat) <= bw(rcm) else (rcm, bw(rcm))
+
+    keep = np.ones(n, bool)
+    perm, w = order(keep)
+    full = (perm, w)
+    if w <= max_w:
+        return np.zeros(0, int), perm, w
+    cnt = np.diff(A.indptr)
+    for _ in range(max_k):
+        keep[int(np.argmax(np.where(keep, cnt, -1)))] = False
+        perm, w = order(keep)
+        if w <= max_w:
+            return np.flatnonzero(~keep), perm, w
+    return np.zeros(0, int), full[0], full[1]

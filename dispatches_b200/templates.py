@@ -504,6 +504,106 @@ def solar_battery_hydrogen(T: int, batt_mw=0.0, batt_mwh=0.0, pem_mw=0.0, tank_k
     return B.build(equilibrate=True)         # holdups (1e6 mol) next to powers (1e5 kW) and flows (1e2 mol/s)
 
 
+SOLAR_SIZE_COLUMNS = ("pv_add_system_capacity", "battery_system_capacity", "battery_system_energy", "pem_system_capacity",
+                      "h2_tank_size", "turb_system_capacity")
+
+
+def solar_battery_hydrogen_design(T: int, pv_cfs, pv_mw=0.0, turb_mw=0.0, reserve_mw=100.0, max_sales=1000.0, max_purchases=1000.0,
+                                  par=None) -> LPTemplate:
+    """pv_battery_hydrogen_optimize with design_opt=True (size_constraints, solar_battery_hydrogen.py:205-236): the six sizes
+    (added PV, battery power / energy, PEM, tank, turbine) are columns of their own, each in a ``<=`` row of every period.  Those six
+    columns make A A' dense (half bandwidth 225 at T = 24), so the band kernels cannot take this template;
+    ``lp_template.find_linking_columns`` finds exactly these six, and without them the half bandwidth is 31 (DESIGN §2 row (f)).
+    The PV capacity factors multiply the added-PV column, so the PV series is part of the template; the batch runs over
+    cparams = lmp[T] and rparams = load_kw[T].
+
+    Presolve against the raw LP: arcs substituted as in ``solar_battery_hydrogen``; the per-period nameplate power / energy and PV
+    capacity copies replaced by the size columns they are bounded by (nothing else prices them, so they sit at the size); the
+    capacity requirement (:352, repeated in every period) kept once; pv.electricity substituted by the splitter balance; the two
+    turbine ramp rows of a period as one ranged row; turb_max_p (:231) dropped, turbine_reserve_lb2 implies it (reserve >= 0); the
+    size bounds of 1e7 / 1e8 kW and the hydrogen-flow bound of the PEM (3.6e7 kW) dropped: they never bind at a size anyone pays for,
+    and next to kW-scale flows they would set the scale of the whole LP; the cyclic chain of nameplate-power links (:47, :61) is gone with
+    the copies, so none of its redundant links remains; grid_sales - grid_purchase <= max_sales is implied by the bounds."""
+    P = dict(SOLAR); P.update(par or {})
+    cf = np.asarray(pv_cfs, float).reshape(T)
+    reserve = np.broadcast_to(np.asarray(reserve_mw, float), (T,))
+    pv_base, turb_base = pv_mw * 1e3, turb_mw * 1e3
+    k_turb = P["s_per_ts"] / H2_MOLS_PER_KG * P["h2_turb_conv"]
+    k_res = P["h2_turb_conv"] / H2_MOLS_PER_KG
+    k_pem = P["s_per_ts"] * PEM_ELEC_TO_MOL
+    ramp = P["turbine_ramp_mw_per_min"] * 1e3
+    fmax = P["flow_mol_ub"]
+    B = TemplateBuilder(f"solar_battery_hydrogen_design_T{T}", Pc=T, Pr=T)
+    ann = 52.143 / (T / 168.0)
+    kk = 1e-3 * PA * ann
+    Va = B.var("pv_add_system_capacity")
+    Bc = B.var("battery_system_capacity")
+    Be = B.var("battery_system_energy")
+    Pc = B.var("pem_system_capacity")
+    Ts = B.var("h2_tank_size")
+    Tc = B.var("turb_system_capacity", lb=turb_base)
+    B.cost(Va, 1e-3 * (P["pv_cap_cost"] + PA * P["pv_op_cost"]))
+    B.cost(Bc, 1e-3 * P["batt_cap_cost_kw"]); B.cost(Be, 1e-3 * P["batt_cap_cost_kwh"])
+    B.cost(Pc, 1e-3 * (P["pem_cap_cost"] + PA * P["pem_op_cost"]))
+    B.cost(Ts, 1e-3 * (P["tank_cap_cost_per_kg"] + PA * P["tank_op_cost"]))
+    B.cost(Tc, 1e-3 * (P["turbine_cap_cost"] + PA * P["turbine_op_cost"]))
+    B.obj_const(1e-3 * (PA * pv_base * P["pv_op_cost"] - P["turbine_cap_cost"] * turb_base))
+    g, pe, i, o, s, br, tt, tp, hd, gp, gs, tr = ({} for _ in range(12))
+    for t in range(T):
+        p = f"blk[{t}].fs."
+        g[t] = B.var(p + "splitter.grid_elec[0]")
+        pe[t] = B.var(p + "pem.electricity[0]")
+        i[t] = B.var(p + "battery.elec_in[0]")
+        o[t] = B.var(p + "battery.elec_out[0]")
+        s[t] = B.var(p + "battery.state_of_charge[0]")
+        br[t] = B.var(f"blk[{t}].battery_reserve")
+        tt[t] = B.var(p + "h2_tank.outlet_to_turbine.flow_mol[0]", lb=P["turbine_min_mw"] * 1e3 / k_turb, ub=fmax)
+        tp[t] = B.var(p + "h2_tank.outlet_to_pipeline.flow_mol[0]", ub=fmax)
+        hd[t] = B.var(p + "h2_tank.tank_holdup[0]")
+        gp[t] = B.var(f"blk[{t}].grid_purchase", ub=max_purchases * 1e3)
+        gs[t] = B.var(f"blk[{t}].grid_sales", ub=max_sales * 1e3)
+        tr[t] = B.var(f"blk[{t}].turbine_reserve")
+        B.cost(gs[t], (0.0, {t: -kk * 1e-3})); B.cost(gp[t], (0.0, {t: kk * 1e-3}))
+        B.cost(pe[t], kk * P["pem_var_cost"])
+        B.cost(tt[t], kk * P["turbine_var_cost"] * k_turb)
+        B.cost(tp[t], -kk * P["h2_price_per_kg"] / H2_MOLS_PER_KG * P["s_per_ts"])
+    for t in range(T):
+        tm = (t - 1) % T
+        pv = {g[t]: 1.0, pe[t]: 1.0, i[t]: 1.0}                       # pv.electricity = grid + PEM + battery (elec_splitter.py:115-117)
+        B.le(f"pv_max[{t}]", {**pv, Va: -cf[t]} if cf[t] != 0.0 else pv, cf[t] * pv_base)                      # solar_pv.py:82-84
+        row = {s[t]: 1.0, i[t]: -ETA_C, o[t]: 1.0 / ETA_D}
+        row[s[tm]] = row.get(s[tm], 0.0) - 1.0
+        B.eq(f"soc[{t}]", row)
+        B.le(f"soc_max[{t}]", {s[t]: 1.0, Be: -1.0})                                         # battery.py:155-157, :225-226
+        B.le(f"charge_max[{t}]", {i[t]: 1.0, Bc: -1.0})
+        B.le(f"discharge_max[{t}]", {o[t]: 1.0, Bc: -1.0})
+        B.le(f"battery_reserve_lb1[{t}]", {br[t]: 1.0, Bc: -1.0})
+        B.le(f"battery_reserve_lb2[{t}]", {br[t]: 1.0, s[t]: -1.0})
+        B.le(f"pem_max_p[{t}]", {pe[t]: 1.0, Pc: -1.0})                                      # :229
+        row = {hd[t]: 1.0, tp[t]: P["s_per_ts"], tt[t]: P["s_per_ts"], pe[t]: -k_pem}
+        row[hd[tm]] = row.get(hd[tm], 0.0) - 1.0
+        B.eq(f"tank[{t}]", row)
+        B.le(f"tank_max_p[{t}]", {hd[t]: 1.0 / H2_MOLS_PER_KG, Ts: -1.0})                    # :230
+        B.eq(f"meet_load[{t}]", {g[t]: 1.0, o[t]: 1.0, tt[t]: k_turb, gp[t]: 1.0, gs[t]: -1.0}, (0.0, {t: 1.0}))
+        B.le(f"turbine_reserve_lb1[{t}]", {tr[t]: 1.0, hd[t]: -k_res})
+        B.le(f"turbine_reserve_lb2[{t}]", {tr[t]: 1.0, tt[t]: k_turb, Tc: -1.0})
+        r1 = (max(reserve[max(t - 1, 0):t]) if t > 0 else reserve[0]) * 1e3
+        row = {br[t]: -1.0, tr[t]: -1.0, g[t]: 1.0, i[t]: 1.0}                       # PV headroom C cf - w with w substituted
+        if cf[t] != 0.0:
+            row[Va] = -cf[t]
+        B.le(f"min_reserve[{t}]", row, -r1 + cf[t] * pv_base)
+        if T > 1:                                                                            # both ramp rows (:323-324) as one ranged row
+            rr = B.var(f"ramp_range[{t}]", ub=2.0 * ramp)
+            B.eq(f"energy_ramp[{t}]", {tt[t]: k_turb, tt[tm]: -k_turb, rr: 1.0}, ramp)
+    B.le("battery_min_duration", {Bc: 0.5, Be: -1.0})                                        # :234-235
+    B.le("battery_max_duration", {Be: 1.0, Bc: -8.0})
+    B.le("capacity_requirement", {Bc: -P["capacity_credit_battery"], Tc: -1.0}, -P["capacity_requirement"] * 1e3)
+    B.meta.update(kind="solar_battery_hydrogen_design", T=T, ann=ann, k_turb=k_turb, pv_base=pv_base, turb_base=turb_base, pv_cfs=cf.copy())
+    # not equilibrated: the six size columns sit in rows of every period, and the geometric-mean row / column scaling then stretches
+    # the bounds and costs over 1e-8 .. 1e11 (the interior-point iterates diverge); in kW, mol and $ the LP solves in about 22 iterations
+    return B.build(equilibrate=False)
+
+
 def solar_rparams(T, pv_cfs, pv_mw, load_mw):
     """rparams rows of solar_battery_hydrogen: [pv_kw*cf_t (T), load_kw_t (T), pv_kw]; pv_cfs / load_mw [T] or [N, T], pv_mw scalar or [N]"""
     cf = np.atleast_2d(np.asarray(pv_cfs, float)); ld = np.atleast_2d(np.asarray(load_mw, float))
