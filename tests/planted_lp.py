@@ -232,6 +232,13 @@ def optimality(p: PlantedLP, k):
         n_basic=int(inside.sum()))
 
 
+def rel(a, ref):
+    """largest |a - ref| of each LP relative to that LP's |ref|_inf (absolute where ref = 0): basic columns are >= 1 and bounds >= 2
+    unless a test scales the data down, so this is 1e-6 * max(1, |x*|) of the planted LPs and as tight on scaled ones"""
+    s = np.abs(ref).max(1)
+    return float((np.abs(a - ref).max(1) / np.where(s > 0, s, 1.0)).max(initial=0.0))
+
+
 def shuffled(t: LPTemplate, seed):
     """the same LPs with rows and columns in a random caller order (for dsp_lp_template_create_csr, whose own ordering and
     xperm / yperm write-back then matter).  Returns (template, column order, row order): column j of the new template is column

@@ -14,6 +14,7 @@ import torch
 
 from dispatches_b200 import solver as S
 from planted_lp import AMAP_CASES, CASES, VARIANTS, band_placement, placement_of_launch, planted, shuffled
+from planted_lp import rel as _rel
 
 pytestmark = pytest.mark.gpu
 
@@ -50,13 +51,6 @@ def _solver(p, native):
         t, cperm, rperm = shuffled(p.t, seed=7)
         return S.BatchLPSolver(t, native_setup=True), cperm, rperm
     return S.BatchLPSolver(p.t), None, None
-
-
-def _rel(a, ref):
-    """largest |a - ref| of each LP relative to that LP's |ref|_inf (absolute where ref = 0): basic columns are >= 1 and bounds >= 2
-    unless a test scales the data down, so this is 1e-6 * max(1, |x*|) of the planted LPs and as tight on scaled ones"""
-    s = np.abs(ref).max(1)
-    return float((np.abs(a - ref).max(1) / np.where(s > 0, s, 1.0)).max())
 
 
 def _check(p, r, cperm=None, rperm=None, what=""):
