@@ -113,7 +113,8 @@ int dsp_lp_template_set_stage_chain1(dsp_template *t, const dsp_stage_chain1_des
  * the complementarity gap has converged (< tol) while residuals / gap sit at the rounding floor of the ill-conditioned normal
  * equations, residuals < 10 feas_tol and gap < 10 tol; OR complementarity < 1e-3 tol with residuals < 100 feas_tol and
  * gap < 1000 tol (the effective worst-case tolerance is therefore 1000 tol = 1e-6 relative on the LP part of the objective at
- * the defaults).  DSP_INFEASIBLE is reported only for a negative
+ * the defaults).  The stage-2 kernel's two looser branches also require |A x - b| < 10 feas_tol relative to the primal scale
+ * itself, not to 1 + the scaled |b|.  DSP_INFEASIBLE is reported only for a negative
  * upper bound produced by Umap / rparams; other infeasible / unbounded LPs end as DSP_MAX_ITER / DSP_NUMERICAL.  Every kernel
  * applies one rule: u_j < -1e-9 * beta_b is infeasible, where beta_b = max(max_i |b_i|, max_j u_j) (1 if that is <= 0) is the
  * LP's primal scale; a bound above that is clamped to 0 and the LP is solved (the 1e-9 is a rounding margin, far inside the 1e-7
