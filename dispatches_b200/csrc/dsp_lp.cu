@@ -14,6 +14,9 @@
 //   * FP64 throughout (cond(M) reaches 1e15 near convergence, SURVEY.md §0.6);
 //   * Mehrotra predictor-corrector; M is factorised once per iteration by a band LDL' (half bandwidth w),
 //     two band solves per iteration.  The numpy mirror of exactly this algorithm is oracle/ipm_numpy.py.
+//
+// Kernel `dsp_ipm_dense_kernel` (any bandwidth, m <= 1024; dsp_lp_template_create_dense or DSP_KERNEL_DENSE): the same iteration,
+// one CTA per LP, M = A D A' dense in a workspace, blocked LDL' with FP64 tensor-core trailing updates (dsp_dense.cuh).
 #include "dsp_lp.h"
 
 #include <cuda_runtime.h>
@@ -491,6 +494,360 @@ __global__ void __launch_bounds__(kMaxWarps * 32, 1) dsp_ipm_band_kernel(const K
 
 }  // namespace
 
+#include "dsp_dense.cuh"
+
+namespace {
+// =====================================================================================================
+// Dense kernel `dsp_ipm_dense_kernel` (any bandwidth, m <= 1024): one persistent CTA of kDenseWarps warps per LP, the same
+// Mehrotra iteration as the band kernel's solve_one with its element-wise and CSR passes spread over the CTA; M = A D A' dense,
+// factored by the blocked LDL' of dsp_dense.cuh in a per-CTA workspace region.  Numpy mirror: oracle/ipm_dense_numpy.py.
+// =====================================================================================================
+constexpr int kDenseWarps = 8;
+constexpr int kDenseThreads = kDenseWarps * 32;
+constexpr int kDenseMaxM = 1024;
+
+struct DParams {
+    int m, n, nb, Pc, Pr, nt;
+    const double *c0, *b0, *u0, *omap, *ocmap;
+    const int *cm_ptr, *cm_idx, *bm_ptr, *bm_idx, *um_ptr, *um_idx;
+    const double *cm_val, *bm_val, *um_val;
+    double o0;
+    const int *A_ptr, *A_idx, *At_ptr, *At_idx;
+    const double *A_val, *At_val;
+    int nent;                          // entries of the lower pattern of A A', tile-major
+    const int *asm_pos, *asm_ptr, *asm_col;   // workspace offset of entry e; its products asm_val[asm_ptr[e] ..] * d[asm_col[..]]
+    const double *asm_val;
+    long long N;
+    const double *cparams, *rparams;
+    long long rstride;
+    double tol, feas_tol, step_frac, reg;
+    int max_iter;
+    double *obj, *x_out, *y_out;
+    int *status, *iters;
+    unsigned long long *ticket;
+    const int *xperm, *yperm;
+    double *ws;                        // per-CTA regions: the lower tiles of M, then (vec_in_smem == 0) the per-LP vectors
+    long long cta_doubles;
+    int vec_in_smem;
+};
+
+// doubles of the per-LP vectors: x z c rd d dx cor rx (n), s wv u ru cors rs (nb), y b rp (m), dy dinv (mp)
+inline long long dense_vec_doubles(int m, int n, int nb, int nt) { return 8LL * n + 6LL * nb + 3LL * m + 2LL * nt * dense::TS; }
+// shared memory ahead of the vectors: reduction slots and the ticket, the two staged-tile buffers
+constexpr size_t kDenseSmemFixed = (size_t)(2 * kDenseWarps + 2 * dense::TS * dense::LDS) * 8;
+
+struct DWork {
+    double *x, *z, *c, *rd, *d, *dx, *cor, *rx;
+    double *s, *wv, *u, *ru, *cors, *rs;
+    double *y, *b, *rp;
+    double *dy, *dinv;                 // mp
+    double *G;                         // lower tiles of M
+    double *SA, *SB, *red;
+};
+
+__device__ __forceinline__ double cta_max(double v, double *red) {
+    v = warp_max(v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double r = red[0];
+#pragma unroll
+    for (int w = 1; w < kDenseWarps; ++w) r = fmax(r, red[w]);
+    return r;
+}
+__device__ __forceinline__ double cta_sum(double v, double *red) {
+    v = warp_sum(v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double r = red[0];
+#pragma unroll
+    for (int w = 1; w < kDenseWarps; ++w) r += red[w];
+    return r;
+}
+
+template <bool CORR>
+__device__ void dense_newton(const DWork &W, const DParams &P, double smu, int tid) {
+    const int n = P.n, nb = P.nb, m = P.m, mp = P.nt * dense::TS;
+    for (int j = tid; j < nb; j += kDenseThreads) {
+        const double wj = W.wv[j];
+        double h = W.rd[j] + W.z[j], as = -wj * W.ru[j];
+        if (CORR) { h -= (smu - W.cor[j]) * W.rx[j]; as += smu - W.cors[j]; }
+        h += as * W.rs[j] - wj;
+        W.dx[j] = W.d[j] * h;
+    }
+    for (int j = nb + tid; j < n; j += kDenseThreads) {
+        double h = W.rd[j] + W.z[j];
+        if (CORR) h -= (smu - W.cor[j]) * W.rx[j];
+        W.dx[j] = W.d[j] * h;
+    }
+    __syncthreads();
+    for (int i = tid; i < mp; i += kDenseThreads) {
+        double acc = 0.0;
+        if (i < m) {
+            acc = W.rp[i];
+            for (int q = P.A_ptr[i]; q < P.A_ptr[i + 1]; ++q) acc += P.A_val[q] * W.dx[P.A_idx[q]];
+        }
+        W.dy[i] = acc;
+    }
+    __syncthreads();
+    dense::solve(W.G, P.nt, W.dinv, W.dy, tid >> 5, kDenseWarps, tid & 31);
+    for (int j = tid; j < n; j += kDenseThreads) {
+        double acc = 0.0;
+        for (int q = P.At_ptr[j]; q < P.At_ptr[j + 1]; ++q) acc += P.At_val[q] * W.dy[P.At_idx[q]];
+        W.dx[j] = W.d[j] * acc - W.dx[j];
+    }
+    __syncthreads();
+}
+
+template <bool CORR>
+__device__ __forceinline__ void dense_step_pass(const DWork &W, const DParams &P, double smu, int tid, double &ip, double &id) {
+    const int n = P.n, nb = P.nb;
+    for (int j = tid; j < nb; j += kDenseThreads) {
+        const double zj = W.z[j], wj = W.wv[j], rxj = W.rx[j], rsj = W.rs[j], dxj = W.dx[j];
+        double dzj = -zj - zj * dxj * rxj;
+        const double dsj = W.ru[j] - dxj;
+        double dwj = -wj - wj * dsj * rsj;
+        if (CORR) { dzj += (smu - W.cor[j]) * rxj; dwj += (smu - W.cors[j]) * rsj; }
+        ip = dmaxd(ip, dmaxd(-dxj * rxj, -dsj * rsj));
+        id = dmaxd(id, dmaxd(-dzj * frcpd(zj), -dwj * frcpd(wj)));
+    }
+    for (int j = nb + tid; j < n; j += kDenseThreads) {
+        const double zj = W.z[j], rxj = W.rx[j], dxj = W.dx[j];
+        double dzj = -zj - zj * dxj * rxj;
+        if (CORR) dzj += (smu - W.cor[j]) * rxj;
+        ip = dmaxd(ip, -dxj * rxj);
+        id = dmaxd(id, -dzj * frcpd(zj));
+    }
+}
+
+// one attempt on LP p: the band kernel's solve_one (same scaling, start point, proximal term, stopping rule, results rules)
+__device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, double step_frac, double reg, int it0, int *status_out,
+                                int *iters_out) {
+    const int n = P.n, nb = P.nb, m = P.m, nt = P.nt, mp = nt * dense::TS;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const double *cp = P.cparams + p * (long long)P.Pc;
+    const double *rp_ = P.rparams + p * P.rstride;
+    double cmax = 0.0, bmax = 0.0, kconst = 0.0;
+    for (int j = tid; j < n; j += kDenseThreads) {
+        double acc = P.c0[j];
+        for (int q = P.cm_ptr[j]; q < P.cm_ptr[j + 1]; ++q) acc += P.cm_val[q] * cp[P.cm_idx[q]];
+        W.c[j] = acc;
+        cmax = dmaxd(cmax, fabs(acc));
+    }
+    for (int i = tid; i < m; i += kDenseThreads) {
+        double acc = P.b0[i];
+        for (int q = P.bm_ptr[i]; q < P.bm_ptr[i + 1]; ++q) acc += P.bm_val[q] * rp_[P.bm_idx[q]];
+        W.b[i] = acc;
+        bmax = dmaxd(bmax, fabs(acc));
+    }
+    for (int j = tid; j < nb; j += kDenseThreads) {
+        double acc = P.u0[j];
+        for (int q = P.um_ptr[j]; q < P.um_ptr[j + 1]; ++q) acc += P.um_val[q] * rp_[P.um_idx[q]];
+        W.u[j] = acc;
+        bmax = dmaxd(bmax, acc);
+    }
+    for (int r = tid; r < P.Pr; r += kDenseThreads) kconst += P.omap[r] * rp_[r];
+    for (int r = tid; r < P.Pc; r += kDenseThreads) kconst += P.ocmap[r] * cp[r];
+    kconst = cta_sum(kconst, W.red) + P.o0;
+    cmax = cta_max(cmax, W.red);
+    bmax = cta_max(bmax, W.red);
+    const double beta_b = bmax > 0.0 ? bmax : 1.0;
+    const double beta_c = cmax > 0.0 ? cmax : 1.0;
+    double bsmax = 0.0;
+    int bad_u = 0;
+    for (int i = tid; i < m; i += kDenseThreads) {
+        const double v = W.b[i] / beta_b;
+        W.b[i] = v;
+        W.y[i] = 0.0;
+        bsmax = dmaxd(bsmax, fabs(v));
+    }
+    for (int j = tid; j < n; j += kDenseThreads) {
+        W.c[j] = W.c[j] / beta_c;
+        double xj = 1.0;
+        if (j < nb) {
+            bad_u |= W.u[j] < -1e-9 * beta_b;
+            const double uj = dmaxd(W.u[j] / beta_b, 1e-10);
+            W.u[j] = uj;
+            xj = fmin(1.0, 0.5 * uj);
+            W.s[j] = uj - xj;
+            W.wv[j] = 1.0;
+        }
+        W.x[j] = xj;
+        W.z[j] = 1.0;
+    }
+    bsmax = cta_max(bsmax, W.red);
+    const double nrm_b = 1.0 + bsmax, nrm_c = 1.0 + (cmax > 0.0 ? 1.0 : 0.0);
+    const double ntot = (double)(n + nb);
+    if (__syncthreads_or(bad_u)) {
+        if (tid == 0) { P.obj[p] = __longlong_as_double(0x7ff8000000000000LL); P.status[p] = DSP_INFEASIBLE; P.iters[p] = it0; }
+        dsp_nan_rows(P.x_out, n, P.y_out, m, p, tid, kDenseThreads);
+        *status_out = DSP_OPTIMAL;          // no second attempt
+        *iters_out = it0;
+        return;
+    }
+    const long long ntd = dense::tiles_doubles(nt);
+    int status = DSP_MAX_ITER, it = 0;
+    double pobj = 0.0;
+    for (it = 0; it <= P.max_iter; ++it) {
+        double pmax = 0.0, dmax = 0.0, musum = 0.0, po = 0.0, dobj = 0.0;
+        for (int i = tid; i < m; i += kDenseThreads) {
+            double acc = W.b[i];
+            for (int q = P.A_ptr[i]; q < P.A_ptr[i + 1]; ++q) acc -= P.A_val[q] * W.x[P.A_idx[q]];
+            W.rp[i] = acc;
+            pmax = dmaxd(pmax, fabs(acc));
+            dobj += W.b[i] * W.y[i];
+        }
+        for (int j = tid; j < n; j += kDenseThreads) {
+            const double xj = W.x[j], zj = W.z[j];
+            double acc = W.c[j] - zj;
+            for (int q = P.At_ptr[j]; q < P.At_ptr[j + 1]; ++q) acc -= P.At_val[q] * W.y[P.At_idx[q]];
+            const double rxj = frcpd(xj);
+            double t = zj * rxj + (xj > 1.0 ? reg * rxj * rxj : reg);
+            if (j < nb) {
+                const double sj = W.s[j], wj = W.wv[j], uj = W.u[j];
+                acc += wj;
+                const double r = uj - xj - sj;
+                const double rsj = frcpd(sj);
+                W.ru[j] = r;
+                W.rs[j] = rsj;
+                pmax = dmaxd(pmax, fabs(r));
+                musum += sj * wj;
+                dobj -= uj * wj;
+                t += wj * rsj;
+            }
+            W.rx[j] = rxj;
+            W.rd[j] = acc;
+            W.d[j] = frcpd(t);
+            dmax = dmaxd(dmax, fabs(acc));
+            musum += xj * zj;
+            po += W.c[j] * xj;
+        }
+        pmax = cta_max(pmax, W.red);
+        dmax = cta_max(dmax, W.red);
+        musum = cta_sum(musum, W.red);
+        po = cta_sum(po, W.red);
+        dobj = cta_sum(dobj, W.red);
+        pobj = po;
+        const double mu = musum / ntot;
+        const double gap = fabs(po - dobj) / dmaxd(kGapFloor, fabs(po));
+        if (!(mu == mu) || !(po == po) || mu > 1e100) { status = DSP_NUMERICAL; break; }
+        const double res = dmaxd(pmax / nrm_b, dmax / nrm_c);
+        const double cgap = ntot * mu / dmaxd(kGapFloor, fabs(po));
+        if (res < P.feas_tol && gap < P.tol) { status = DSP_OPTIMAL; break; }
+        if (cgap < P.tol && res < 10.0 * P.feas_tol && gap < 10.0 * P.tol) { status = DSP_OPTIMAL; break; }
+        if (cgap < 1e-3 * P.tol) {
+            status = (res < 100.0 * P.feas_tol && gap < 1000.0 * P.tol) ? DSP_OPTIMAL : DSP_NUMERICAL;
+            break;
+        }
+        if (it == P.max_iter) break;
+        // ---- assemble the lower tiles of M = A D A' (padding rows: decoupled unit rows) and factor them
+        for (long long e = tid; e < ntd; e += kDenseThreads) W.G[e] = 0.0;
+        __syncthreads();
+        for (int e = tid; e < P.nent; e += kDenseThreads) {
+            double acc = 0.0;
+            for (int q = P.asm_ptr[e]; q < P.asm_ptr[e + 1]; ++q) acc += P.asm_val[q] * W.d[P.asm_col[q]];
+            W.G[P.asm_pos[e]] = acc;
+        }
+        for (int i = m + tid; i < mp; i += kDenseThreads)
+            W.G[(long long)dense::tile_index(i / dense::TS, i / dense::TS) * dense::TILE + (i % dense::TS) * (dense::TS + 1)] = 1.0;
+        dense::factor(W.G, nt, W.SA, W.SB, W.dinv, warp, kDenseWarps, lane);
+        // ---- affine predictor
+        dense_newton<false>(W, P, 0.0, tid);
+        double ip = 0.0, id = 0.0;
+        dense_step_pass<false>(W, P, 0.0, tid, ip, id);
+        ip = cta_max(ip, W.red); id = cta_max(id, W.red);
+        double ap = ip > 1.0 ? 1.0 / ip : 1.0, ad = id > 1.0 ? 1.0 / id : 1.0;
+        double mua = 0.0;
+        for (int j = tid; j < n; j += kDenseThreads) {
+            const double xj = W.x[j], zj = W.z[j], dxj = W.dx[j];
+            const double dzj = -zj - zj * dxj * W.rx[j];
+            mua += (xj + ap * dxj) * (zj + ad * dzj);
+            W.cor[j] = dxj * dzj;
+            if (j < nb) {
+                const double sj = W.s[j], wj = W.wv[j];
+                const double dsj = W.ru[j] - dxj;
+                const double dwj = -wj - wj * dsj * W.rs[j];
+                mua += (sj + ap * dsj) * (wj + ad * dwj);
+                W.cors[j] = dsj * dwj;
+            }
+        }
+        mua = cta_sum(mua, W.red) / ntot;
+        const double sg = mua / mu;
+        const double smu = sg * sg * sg * mu;
+        // ---- centring corrector
+        dense_newton<true>(W, P, smu, tid);
+        ip = 0.0; id = 0.0;
+        dense_step_pass<true>(W, P, smu, tid, ip, id);
+        ip = cta_max(ip, W.red); id = cta_max(id, W.red);
+        ap = step_frac < ip ? step_frac / ip : 1.0;
+        ad = step_frac < id ? step_frac / id : 1.0;
+        for (int j = tid; j < n; j += kDenseThreads) {
+            const double xj = W.x[j], zj = W.z[j], dxj = W.dx[j], rxj = W.rx[j];
+            const double dzj = (smu - W.cor[j]) * rxj - zj - zj * dxj * rxj;
+            if (j < nb) {
+                const double sj = W.s[j], wj = W.wv[j], rsj = W.rs[j];
+                const double dsj = W.ru[j] - dxj;
+                const double dwj = (smu - W.cors[j]) * rsj - wj - wj * dsj * rsj;
+                W.s[j] = sj + ap * dsj;
+                W.wv[j] = wj + ad * dwj;
+            }
+            W.x[j] = xj + ap * dxj;
+            W.z[j] = zj + ad * dzj;
+        }
+        for (int i = tid; i < m; i += kDenseThreads) W.y[i] += ad * W.dy[i];
+        __syncthreads();
+    }
+    // ---- results
+    if (tid == 0) {
+        P.obj[p] = pobj * beta_b * beta_c + kconst;
+        P.status[p] = status;
+        P.iters[p] = it + it0;
+    }
+    if (P.x_out) {
+        double *xo = P.x_out + p * (long long)n;
+        if (P.xperm) { for (int j = tid; j < n; j += kDenseThreads) xo[P.xperm[j]] = W.x[j] * beta_b; }
+        else { for (int j = tid; j < n; j += kDenseThreads) xo[j] = W.x[j] * beta_b; }
+    }
+    if (P.y_out) {
+        double *yo = P.y_out + p * (long long)m;
+        if (P.yperm) { for (int i = tid; i < m; i += kDenseThreads) yo[P.yperm[i]] = W.y[i] * beta_c; }
+        else { for (int i = tid; i < m; i += kDenseThreads) yo[i] = W.y[i] * beta_c; }
+    }
+    __syncthreads();
+    *status_out = status;
+    *iters_out = it + it0;
+}
+
+__global__ void __launch_bounds__(kDenseThreads, 1) dsp_ipm_dense_kernel(const DParams P) {
+    extern __shared__ __align__(16) double dsm[];
+    unsigned long long &ticket = *(unsigned long long *)(dsm + kDenseWarps);     // behind the reduction slots
+    DWork W;
+    W.red = dsm;
+    W.SA = dsm + 2 * kDenseWarps;
+    W.SB = W.SA + dense::TS * dense::LDS;
+    const int n = P.n, nb = P.nb, m = P.m, mp = P.nt * dense::TS;
+    W.G = P.ws + (long long)blockIdx.x * P.cta_doubles;
+    double *base = P.vec_in_smem ? W.SB + dense::TS * dense::LDS : W.G + dense::tiles_doubles(P.nt);
+    W.x = base; W.z = W.x + n; W.c = W.z + n; W.rd = W.c + n; W.d = W.rd + n; W.dx = W.d + n; W.cor = W.dx + n; W.rx = W.cor + n;
+    W.s = W.rx + n; W.wv = W.s + nb; W.u = W.wv + nb; W.ru = W.u + nb; W.cors = W.ru + nb; W.rs = W.cors + nb;
+    W.y = W.rs + nb; W.b = W.y + m; W.rp = W.b + m;
+    W.dy = W.rp + m; W.dinv = W.dy + mp;
+    for (;;) {
+        if (threadIdx.x == 0) ticket = atomicAdd(P.ticket, 1ULL);
+        __syncthreads();
+        const unsigned long long t = ticket;
+        __syncthreads();
+        if ((long long)t >= P.N) break;
+        int st, it0 = 0;
+        // second attempt (shorter step, stronger proximal term) for the rare LP whose first attempt ends non-optimal
+        dense_solve_one(W, P, (long long)t, P.step_frac, P.reg, 0, &st, &it0);
+        if (st != DSP_OPTIMAL) dense_solve_one(W, P, (long long)t, 0.99, 10.0 * P.reg, it0, &st, &it0);
+    }
+}
+
+}  // namespace
+
 namespace {
 #include "dsp_stage_wb.cuh"
 
@@ -648,6 +1005,14 @@ struct dsp_template {
     int64_t cap_rp_rows;
     cudaStream_t stream, stream2;
     std::atomic<int> busy;         // a host call is in flight on this handle (staging buffers, streams and ticket are per handle)
+    bool dense_only;               // made by dsp_lp_template_create_dense: no band data, only the dense kernel runs
+    struct Dense {                 // the dense kernel's data (dense templates; band templates: built at the first DSP_KERNEL_DENSE call)
+        bool ready;
+        int nt, nent;
+        const int *A_ptr, *A_idx, *At_ptr, *At_idx, *asm_pos, *asm_ptr, *asm_col;
+        const double *A_val, *At_val, *asm_val;
+    };
+    mutable Dense dn;
 };
 
 namespace {
@@ -699,6 +1064,151 @@ template <class F>
 int allow_smem(F fn, size_t bytes) {
     CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     CK(cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    return 0;
+}
+
+int check_maps(const dsp_template_desc *D) {
+    for (int q = 0; q < D->cmap.ptr[D->n]; ++q)
+        if (D->cmap.idx[q] < 0 || D->cmap.idx[q] >= D->Pc) { g_err = "cmap.idx out of range"; return DSP_E_ARG; }
+    for (int q = 0; q < D->bmap.ptr[D->m]; ++q)
+        if (D->bmap.idx[q] < 0 || D->bmap.idx[q] >= D->Pr) { g_err = "bmap.idx out of range"; return DSP_E_ARG; }
+    for (int q = 0; q < D->umap.ptr[D->nb]; ++q)
+        if (D->umap.idx[q] < 0 || D->umap.idx[q] >= D->Pr) { g_err = "umap.idx out of range"; return DSP_E_ARG; }
+    return 0;
+}
+
+// what every template carries whatever its kernels: the device and its limits, the streams, the ticket counter and the
+// parameter maps of c, b, u and the objective constant (D's matrix and assembly fields are not read)
+int template_init(dsp_template *T, const dsp_template_desc *D) {
+    const int m = D->m, n = D->n, nb = D->nb;
+    memset(&T->kp, 0, sizeof(KParams));
+    T->cap_N = 0; T->cap_x = T->cap_y = false; T->cap_rp_rows = 0;
+    T->has_stage = false; T->has_chain1 = false; T->stage_blocks_per_sm = 0; T->ws = nullptr; T->ws_bytes = 0;
+    T->h_cp = T->h_rp = T->h_obj = T->h_x = T->h_y = nullptr; T->h_status = T->h_iters = nullptr;
+    T->d_cp = T->d_rp = T->d_obj = T->d_x = T->d_y = nullptr; T->d_status = T->d_iters = nullptr;
+    T->stream = nullptr; T->stream2 = nullptr; T->busy.store(0);
+    T->dense_only = false;
+    memset(&T->dn, 0, sizeof(T->dn));
+    CK(cudaGetDevice(&T->device));
+    cudaDeviceProp prop;
+    CK(cudaGetDeviceProperties(&prop, T->device));
+    T->sm_count = prop.multiProcessorCount;
+    T->smem_optin = (int)prop.sharedMemPerBlockOptin;
+    T->ws_cap = prop.totalGlobalMem / 4;
+    KParams &K = T->kp;
+    K.m = m; K.n = n; K.nb = nb; K.Pc = D->Pc; K.Pr = D->Pr;
+    K.o0 = D->o0;
+    auto up_d = [&](const double *src, size_t cnt, const double **dst) -> int {
+        std::vector<double> v(src, src + cnt);
+        double *d;
+        int rc = upload(v, &d);
+        if (rc) return rc;
+        T->dev_allocs.push_back(d);
+        *dst = d;
+        return 0;
+    };
+    auto up_i = [&](const int32_t *src, size_t cnt, const int **dst) -> int {
+        std::vector<int> v(src, src + cnt);
+        int *d;
+        int rc = upload(v, &d);
+        if (rc) return rc;
+        T->dev_allocs.push_back(d);
+        *dst = d;
+        return 0;
+    };
+    int rc = 0;
+    rc |= up_d(D->c0, n, &K.c0);
+    rc |= up_d(D->b0, m, &K.b0);
+    rc |= up_d(D->u0, nb, &K.u0);
+    rc |= up_d(D->omap, D->Pr, &K.omap);
+    rc |= up_d(D->ocmap, D->Pc, &K.ocmap);
+    rc |= up_i(D->cmap.ptr, n + 1, &K.cm_ptr);
+    rc |= up_i(D->cmap.idx, D->cmap.ptr[n], &K.cm_idx);
+    rc |= up_d(D->cmap.val, D->cmap.ptr[n], &K.cm_val);
+    rc |= up_i(D->bmap.ptr, m + 1, &K.bm_ptr);
+    rc |= up_i(D->bmap.idx, D->bmap.ptr[m], &K.bm_idx);
+    rc |= up_d(D->bmap.val, D->bmap.ptr[m], &K.bm_val);
+    rc |= up_i(D->umap.ptr, nb + 1, &K.um_ptr);
+    rc |= up_i(D->umap.idx, D->umap.ptr[nb], &K.um_idx);
+    rc |= up_d(D->umap.val, D->umap.ptr[nb], &K.um_val);
+    if (rc) return DSP_E_CUDA;
+    CK(cudaMalloc((void **)&T->ticket, 16 * sizeof(unsigned long long)));
+    T->dev_allocs.push_back(T->ticket);
+    CK(cudaStreamCreateWithFlags(&T->stream, cudaStreamNonBlocking));
+    CK(cudaStreamCreateWithFlags(&T->stream2, cudaStreamNonBlocking));
+    return 0;
+}
+
+// The dense kernel's data for a template whose internal-order CSR is (A_ptr, A_idx, A_val): the CSC, and the assembly list of the
+// lower pattern of A A' in tile-major workspace order -- entry e of M sits at asm_pos[e] and is the sum of
+// asm_val[q] * d[asm_col[q]] over q in [asm_ptr[e], asm_ptr[e+1]).  Host-only analysis, then one upload.
+constexpr long long kDenseMaxTerms = 1LL << 26;
+int dense_build(dsp_template *T, const std::vector<int> &A_ptr, const std::vector<int> &A_idx, const std::vector<double> &A_val) {
+    const int m = T->kp.m, n = T->kp.n, nnz = A_ptr[m];
+    const int TS = dense::TS;
+    std::vector<int> At_ptr(n + 1, 0), At_idx(nnz);
+    std::vector<double> At_val(nnz);
+    for (int q = 0; q < nnz; ++q) At_ptr[A_idx[q] + 1]++;
+    for (int j = 0; j < n; ++j) At_ptr[j + 1] += At_ptr[j];
+    {
+        std::vector<int> fill(At_ptr.begin(), At_ptr.end() - 1);
+        for (int i = 0; i < m; ++i)
+            for (int q = A_ptr[i]; q < A_ptr[i + 1]; ++q) { const int dst = fill[A_idx[q]]++; At_idx[dst] = i; At_val[dst] = A_val[q]; }
+    }
+    long long nterms = 0;
+    for (int j = 0; j < n; ++j) { const long long c = At_ptr[j + 1] - At_ptr[j]; nterms += c * (c + 1) / 2; }
+    if (nterms > kDenseMaxTerms) { g_err = "dense kernel: the assembly list of A A' has more than 2^26 products"; return DSP_E_ARG; }
+    // entries of the lower pattern (a >= b), first seen order; then sorted by workspace position
+    std::vector<int> slot((size_t)m * m, -1), cnt;
+    std::vector<long long> pos;
+    for (int j = 0; j < n; ++j)
+        for (int qa = At_ptr[j]; qa < At_ptr[j + 1]; ++qa)
+            for (int qb = At_ptr[j]; qb <= qa; ++qb) {
+                const int a = At_idx[qa], b = At_idx[qb];      // rows ascending within a column: a >= b
+                int &e = slot[(size_t)a * m + b];
+                if (e < 0) {
+                    e = (int)pos.size();
+                    pos.push_back((long long)dense::tile_index(a / TS, b / TS) * dense::TILE + (a % TS) * TS + (b % TS));
+                    cnt.push_back(0);
+                }
+                cnt[e]++;
+            }
+    const int nent = (int)pos.size();
+    std::vector<int> order(nent), rank(nent);
+    for (int e = 0; e < nent; ++e) order[e] = e;
+    std::sort(order.begin(), order.end(), [&](int x, int y) { return pos[x] < pos[y]; });
+    for (int r = 0; r < nent; ++r) rank[order[r]] = r;
+    std::vector<int> asm_pos(nent), asm_ptr(nent + 1, 0), asm_col((size_t)nterms);
+    std::vector<double> asm_val((size_t)nterms);
+    for (int r = 0; r < nent; ++r) { asm_pos[r] = (int)pos[order[r]]; asm_ptr[r + 1] = asm_ptr[r] + cnt[order[r]]; }
+    std::vector<int> fill(asm_ptr.begin(), asm_ptr.end() - 1);
+    for (int j = 0; j < n; ++j)
+        for (int qa = At_ptr[j]; qa < At_ptr[j + 1]; ++qa)
+            for (int qb = At_ptr[j]; qb <= qa; ++qb) {
+                const int r = rank[slot[(size_t)At_idx[qa] * m + At_idx[qb]]];
+                asm_col[fill[r]] = j;
+                asm_val[fill[r]++] = At_val[qa] * At_val[qb];
+            }
+    dsp_template::Dense &D = T->dn;
+    int *pi; double *pd;
+    auto ui = [&](const std::vector<int> &v, const int **dst) { int rc = upload(v, &pi); if (!rc) { T->dev_allocs.push_back(pi); *dst = pi; } return rc; };
+    auto ud = [&](const std::vector<double> &v, const double **dst) { int rc = upload(v, &pd); if (!rc) { T->dev_allocs.push_back(pd); *dst = pd; } return rc; };
+    int rc = 0;
+    rc = rc ? rc : ui(A_ptr, &D.A_ptr);
+    rc = rc ? rc : ui(A_idx, &D.A_idx);
+    rc = rc ? rc : ud(A_val, &D.A_val);
+    rc = rc ? rc : ui(At_ptr, &D.At_ptr);
+    rc = rc ? rc : ui(At_idx, &D.At_idx);
+    rc = rc ? rc : ud(At_val, &D.At_val);
+    rc = rc ? rc : ui(asm_pos, &D.asm_pos);
+    rc = rc ? rc : ui(asm_ptr, &D.asm_ptr);
+    rc = rc ? rc : ui(asm_col, &D.asm_col);
+    rc = rc ? rc : ud(asm_val, &D.asm_val);
+    if (rc) return rc;
+    CK(cudaFuncSetAttribute(dsp_ipm_dense_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
+    D.nt = (m + TS - 1) / TS;
+    D.nent = nent;
+    D.ready = true;
     return 0;
 }
 }  // namespace
@@ -782,12 +1292,7 @@ int dsp_lp_template_create(const dsp_template_desc *D, dsp_template **out) {
         }
     for (int q = 0; q < nasm; ++q)
         if (D->asm_col[q] < 0 || D->asm_col[q] >= n) { g_err = "asm_col out of range"; return DSP_E_ARG; }
-    for (int q = 0; q < D->cmap.ptr[n]; ++q)
-        if (D->cmap.idx[q] < 0 || D->cmap.idx[q] >= D->Pc) { g_err = "cmap.idx out of range"; return DSP_E_ARG; }
-    for (int q = 0; q < D->bmap.ptr[m]; ++q)
-        if (D->bmap.idx[q] < 0 || D->bmap.idx[q] >= D->Pr) { g_err = "bmap.idx out of range"; return DSP_E_ARG; }
-    for (int q = 0; q < D->umap.ptr[nb]; ++q)
-        if (D->umap.idx[q] < 0 || D->umap.idx[q] >= D->Pr) { g_err = "umap.idx out of range"; return DSP_E_ARG; }
+    if (int rc = check_maps(D)) return rc;
     // CSC of A
     std::vector<int> At_ptr(n + 1, 0), At_idx(nnz);
     std::vector<double> At_val(nnz);
@@ -829,40 +1334,10 @@ int dsp_lp_template_create(const dsp_template_desc *D, dsp_template **out) {
         dsp_template *t;
         ~Guard() { if (t) dsp_lp_template_destroy(t); }
     } guard{T};
-    memset(&T->kp, 0, sizeof(KParams));
-    T->cap_N = 0; T->cap_x = T->cap_y = false; T->cap_rp_rows = 0;
-    T->has_stage = false; T->has_chain1 = false; T->stage_blocks_per_sm = 0; T->ws = nullptr; T->ws_bytes = 0;
-    T->h_cp = T->h_rp = T->h_obj = T->h_x = T->h_y = nullptr; T->h_status = T->h_iters = nullptr;
-    T->d_cp = T->d_rp = T->d_obj = T->d_x = T->d_y = nullptr; T->d_status = T->d_iters = nullptr;
-    T->stream = nullptr; T->stream2 = nullptr; T->busy.store(0);
-    CK(cudaGetDevice(&T->device));
-    cudaDeviceProp prop;
-    CK(cudaGetDeviceProperties(&prop, T->device));
-    T->sm_count = prop.multiProcessorCount;
-    T->smem_optin = (int)prop.sharedMemPerBlockOptin;
-    T->ws_cap = prop.totalGlobalMem / 4;
+    if (int rc = template_init(T, D)) return rc;
     KParams &K = T->kp;
-    K.m = m; K.n = n; K.nb = nb; K.w = wt; K.Pc = D->Pc; K.Pr = D->Pr; K.nnz = nnz; K.nasm = nasm;
+    K.w = wt; K.nnz = nnz; K.nasm = nasm;
     K.hot_bytes = (int)hot_bytes;
-    K.o0 = D->o0;
-    auto up_d = [&](const double *src, size_t cnt, const double **dst) -> int {
-        std::vector<double> v(src, src + cnt);
-        double *d;
-        int rc = upload(v, &d);
-        if (rc) return rc;
-        T->dev_allocs.push_back(d);
-        *dst = d;
-        return 0;
-    };
-    auto up_i = [&](const int32_t *src, size_t cnt, const int **dst) -> int {
-        std::vector<int> v(src, src + cnt);
-        int *d;
-        int rc = upload(v, &d);
-        if (rc) return rc;
-        T->dev_allocs.push_back(d);
-        *dst = d;
-        return 0;
-    };
     {
         unsigned char *d;
         int rc = upload(hot, &d);
@@ -870,32 +1345,12 @@ int dsp_lp_template_create(const dsp_template_desc *D, dsp_template **out) {
         T->dev_allocs.push_back(d);
         K.hot_g = d;
     }
-    int rc = 0;
-    rc |= up_d(D->c0, n, &K.c0);
-    rc |= up_d(D->b0, m, &K.b0);
-    rc |= up_d(D->u0, nb, &K.u0);
-    rc |= up_d(D->omap, D->Pr, &K.omap);
-    rc |= up_d(D->ocmap, D->Pc, &K.ocmap);
-    rc |= up_i(D->cmap.ptr, n + 1, &K.cm_ptr);
-    rc |= up_i(D->cmap.idx, D->cmap.ptr[n], &K.cm_idx);
-    rc |= up_d(D->cmap.val, D->cmap.ptr[n], &K.cm_val);
-    rc |= up_i(D->bmap.ptr, m + 1, &K.bm_ptr);
-    rc |= up_i(D->bmap.idx, D->bmap.ptr[m], &K.bm_idx);
-    rc |= up_d(D->bmap.val, D->bmap.ptr[m], &K.bm_val);
-    rc |= up_i(D->umap.ptr, nb + 1, &K.um_ptr);
-    rc |= up_i(D->umap.idx, D->umap.ptr[nb], &K.um_idx);
-    rc |= up_d(D->umap.val, D->umap.ptr[nb], &K.um_val);
-    if (rc) return DSP_E_CUDA;
-    CK(cudaMalloc((void **)&T->ticket, 16 * sizeof(unsigned long long)));
-    T->dev_allocs.push_back(T->ticket);
     K.band_doubles = (m + 2 * wt) + (m + 2 * wt) * (wt + 1);
     K.prob_doubles = 8 * n + 6 * nb + 3 * m + K.band_doubles;
     K.hybrid = 0;
     for (int bw = 1; bw <= 32; bw *= 2)
         for (int placement = 0; placement < 3; ++placement)       // workspace, shared memory + staged template, shared memory
             CK(cudaFuncSetAttribute(band_kernel(bw, placement == 0, placement == 1), cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
-    CK(cudaStreamCreateWithFlags(&T->stream, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&T->stream2, cudaStreamNonBlocking));
     guard.t = nullptr;
     *out = T;
     return 0;
@@ -1155,6 +1610,54 @@ static int launch_band(const dsp_template *T, KParams K, cudaStream_t st) {
     return launched(ctas, warps * 32, smem, warps);
 }
 
+// the dense kernel's data of a band template, built from its device copy of A at the first DSP_KERNEL_DENSE call
+static int ensure_dense(const dsp_template *T) {
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lk(mu);
+    const KParams &K = T->kp;
+    if (K.n_amap > 0) { g_err = "dsp_lp_solve_batch: DSP_KERNEL_DENSE does not take per-problem matrix coefficients"; return DSP_E_ARG; }
+    if (T->dn.ready) return 0;
+    if (K.m > kDenseMaxM) { g_err = "dsp_lp_solve_batch: DSP_KERNEL_DENSE needs m <= 1024 (m = " + std::to_string(K.m) + ")"; return DSP_E_ARG; }
+    std::vector<unsigned char> hot(K.hot_bytes);
+    CK(cudaMemcpy(hot.data(), K.hot_g, hot.size(), cudaMemcpyDeviceToHost));
+    const double *val = (const double *)hot.data();
+    const int *ptr = (const int *)(val + 2 * (size_t)K.nnz + K.nasm), *idx = ptr + K.m + 1;
+    return dense_build(const_cast<dsp_template *>(T), std::vector<int>(ptr, ptr + K.m + 1), std::vector<int>(idx, idx + K.nnz),
+                       std::vector<double>(val, val + K.nnz));
+}
+
+// dense kernel: one persistent CTA per LP in flight, as many CTAs per SM as fit; the lower tiles of M of every CTA in the handle's
+// workspace, the per-LP vectors in shared memory when they fit next to the two staged-tile buffers (else behind the tiles)
+static int launch_dense(const dsp_template *T, const KParams &K, cudaStream_t st) {
+    const dsp_template::Dense &D = T->dn;
+    DParams Q;
+    memset(&Q, 0, sizeof(Q));
+    Q.m = K.m; Q.n = K.n; Q.nb = K.nb; Q.Pc = K.Pc; Q.Pr = K.Pr; Q.nt = D.nt;
+    Q.c0 = K.c0; Q.b0 = K.b0; Q.u0 = K.u0; Q.omap = K.omap; Q.ocmap = K.ocmap;
+    Q.cm_ptr = K.cm_ptr; Q.cm_idx = K.cm_idx; Q.cm_val = K.cm_val; Q.bm_ptr = K.bm_ptr; Q.bm_idx = K.bm_idx; Q.bm_val = K.bm_val;
+    Q.um_ptr = K.um_ptr; Q.um_idx = K.um_idx; Q.um_val = K.um_val; Q.o0 = K.o0;
+    Q.A_ptr = D.A_ptr; Q.A_idx = D.A_idx; Q.A_val = D.A_val; Q.At_ptr = D.At_ptr; Q.At_idx = D.At_idx; Q.At_val = D.At_val;
+    Q.nent = D.nent; Q.asm_pos = D.asm_pos; Q.asm_ptr = D.asm_ptr; Q.asm_col = D.asm_col; Q.asm_val = D.asm_val;
+    Q.N = K.N; Q.cparams = K.cparams; Q.rparams = K.rparams; Q.rstride = K.rstride;
+    Q.tol = K.tol; Q.feas_tol = K.feas_tol; Q.step_frac = K.step_frac; Q.reg = K.reg; Q.max_iter = K.max_iter;
+    Q.obj = K.obj; Q.x_out = K.x_out; Q.y_out = K.y_out; Q.status = K.status; Q.iters = K.iters; Q.ticket = K.ticket;
+    Q.xperm = K.xperm; Q.yperm = K.yperm;
+    const long long vec = dense_vec_doubles(K.m, K.n, K.nb, D.nt);
+    Q.vec_in_smem = kDenseSmemFixed + (size_t)vec * 8 <= (size_t)T->smem_optin;
+    const size_t smem = kDenseSmemFixed + (Q.vec_in_smem ? (size_t)vec * 8 : 0);
+    Q.cta_doubles = dense::tiles_doubles(D.nt) + (Q.vec_in_smem ? 0 : vec);
+    int occ = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dsp_ipm_dense_kernel, kDenseThreads, smem));
+    long long ctas = std::min<long long>(K.N, (long long)T->sm_count * std::max(occ, 1));
+    while (ctas > 1 && (size_t)ctas * Q.cta_doubles * 8 > T->ws_cap) ctas /= 2;
+    const int rc = grow_ws(T, (size_t)ctas * Q.cta_doubles * 8, st);
+    if (rc) return rc;
+    Q.ws = T->ws;
+    CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
+    dsp_ipm_dense_kernel<<<(unsigned)ctas, kDenseThreads, smem, st>>>(Q);
+    return launched(ctas, kDenseThreads, smem, 1);
+}
+
 static int launch_batch(const dsp_template *T, int64_t N, const double *cparams, const double *rparams,
                         int64_t rparams_stride, const dsp_opts *opts, double *obj, int32_t *status, int32_t *iters,
                         double *x, double *y, void *cuda_stream, unsigned long long *ticket) {
@@ -1173,6 +1676,15 @@ static int launch_batch(const dsp_template *T, int64_t N, const double *cparams,
     K.obj = obj; K.status = status; K.iters = iters; K.x_out = x; K.y_out = y;
     K.ticket = ticket;
     K.retry_only = 0;
+    if (T->dense_only && o.kernel != DSP_KERNEL_AUTO && o.kernel != DSP_KERNEL_DENSE) {
+        g_err = "dsp_lp_solve_batch: a template made by dsp_lp_template_create_dense runs only the dense kernel (DSP_KERNEL_AUTO or DSP_KERNEL_DENSE)";
+        return DSP_E_ARG;
+    }
+    if (T->dense_only || o.kernel == DSP_KERNEL_DENSE) {
+        const int rc = ensure_dense(T);
+        if (rc) return rc;
+        return launch_dense(T, K, st);
+    }
     const bool stage = o.kernel == DSP_KERNEL_AUTO || o.kernel == DSP_KERNEL_STAGE;
     if (T->has_stage && T->sp.T > kStage2MaxT && stage) {
         const int rc = launch_stage2_long(T, K, st);
@@ -1295,7 +1807,8 @@ static int solve_batch_host_locked(dsp_template *T, int64_t N, const double *cpa
     cudaStream_t sts[2] = {T->stream, T->stream2};
     int64_t dstride = 0;
     // templates that run in global-workspace mode share ONE workspace: no concurrent chunk kernels for them
-    const bool ws_template = band_geometry(T, K).ws || (T->has_stage && T->sp.T > kStage2MaxT);    // (the long stage kernel's workspace too)
+    const bool dense = T->dense_only || (opts && opts->kernel == DSP_KERNEL_DENSE);            // the dense kernel always uses the workspace
+    const bool ws_template = dense || band_geometry(T, K).ws || (T->has_stage && T->sp.T > kStage2MaxT);    // (the long stage kernel's workspace too)
     // Chunks pay when there is something to overlap: the staging memcpy of pageable input (always), or the H2D copy of a batch whose
     // kernel runs for many waves.  A page-locked batch of a few waves goes in ONE piece: the persistent stage kernels fill every SM
     // with one CTA, so two chunk kernels cannot share the chip and each chunk ends in its own thinning tail.
@@ -1547,9 +2060,83 @@ int dsp_lp_template_create_csr(const dsp_lp_desc *D, dsp_template **out) {
     return 0;
 }
 
+int dsp_lp_template_create_dense(const dsp_lp_desc *D, dsp_template **out) {
+    if (!out) { g_err = "dsp_lp_template_create_dense: out is NULL"; return DSP_E_ARG; }
+    if (!D || D->m <= 0 || D->n <= 0 || !D->A_ptr || !D->A_idx || !D->A_val || !D->u0) { g_err = "dsp_lp_template_create_dense: bad descriptor"; return DSP_E_ARG; }
+    if (D->m > kDenseMaxM) {
+        g_err = "dsp_lp_template_create_dense: m = " + std::to_string(D->m) + " rows; the dense kernel takes m <= 1024";
+        return DSP_E_ARG;
+    }
+    const int m = D->m, n = D->n, nnz = D->A_ptr[m];
+    for (int q = 0; q < nnz; ++q)
+        if (D->A_idx[q] < 0 || D->A_idx[q] >= n) { g_err = "dsp_lp_template_create_dense: A_idx out of range"; return DSP_E_ARG; }
+    // internal order: bounded columns first (stable), rows as given (the dense factorisation does not care about bandwidth)
+    std::vector<int> col_perm, row_perm(m);
+    for (int j = 0; j < n; ++j) if (D->u0[j] < 1e300) col_perm.push_back(j);
+    const int nb = (int)col_perm.size();
+    for (int j = 0; j < n; ++j) if (!(D->u0[j] < 1e300)) col_perm.push_back(j);
+    std::vector<int> col_pos(n);
+    for (int k = 0; k < n; ++k) col_pos[col_perm[k]] = k;
+    for (int i = 0; i < m; ++i) row_perm[i] = i;
+    std::vector<int> A_ptr(m + 1, 0), A_idx(nnz);
+    std::vector<double> A_val(nnz);
+    std::vector<int> rmin(n, m), rmax(n, -1);
+    for (int i = 0; i < m; ++i) {
+        std::vector<std::pair<int, double>> ent;
+        for (int q = D->A_ptr[i]; q < D->A_ptr[i + 1]; ++q) {
+            const int j = col_pos[D->A_idx[q]];
+            ent.emplace_back(j, D->A_val[q]);
+            rmin[j] = std::min(rmin[j], i); rmax[j] = std::max(rmax[j], i);
+        }
+        std::sort(ent.begin(), ent.end());
+        A_ptr[i + 1] = A_ptr[i] + (int)ent.size();
+        for (size_t e = 0; e < ent.size(); ++e) { A_idx[A_ptr[i] + e] = ent[e].first; A_val[A_ptr[i] + e] = ent[e].second; }
+    }
+    int w = 0;                         // half bandwidth of A A' in this row order: rows sharing a column are adjacent
+    for (int j = 0; j < n; ++j) if (rmax[j] >= 0) w = std::max(w, rmax[j] - rmin[j]);
+    std::vector<double> c0(n), u0(std::max(nb, 1)), b0(m);
+    for (int k = 0; k < n; ++k) c0[k] = D->c0 ? D->c0[col_perm[k]] : 0.0;
+    for (int k = 0; k < nb; ++k) u0[k] = D->u0[col_perm[k]];
+    for (int i = 0; i < m; ++i) b0[i] = D->b0 ? D->b0[i] : 0.0;
+    std::vector<int> cp, ci, bp, bi, up, ui;
+    std::vector<double> cv, bv, uv;
+    permute_map(D->cmap, col_perm, n, cp, ci, cv);
+    permute_map(D->bmap, row_perm, m, bp, bi, bv);
+    permute_map(D->umap, col_perm, nb, up, ui, uv);
+    std::vector<double> zPr(std::max(D->Pr, 1), 0.0), zPc(std::max(D->Pc, 1), 0.0);
+    auto nz = [](std::vector<int> &v) { if (v.empty()) v.push_back(0); return v.data(); };
+    auto nzd = [](std::vector<double> &v) { if (v.empty()) v.push_back(0.0); return v.data(); };
+    dsp_template_desc d;
+    memset(&d, 0, sizeof(d));
+    d.m = m; d.n = n; d.nb = nb; d.w = w; d.Pc = D->Pc; d.Pr = D->Pr;
+    d.c0 = c0.data(); d.cmap.ptr = cp.data(); d.cmap.idx = nz(ci); d.cmap.val = nzd(cv);
+    d.b0 = b0.data(); d.bmap.ptr = bp.data(); d.bmap.idx = nz(bi); d.bmap.val = nzd(bv);
+    d.u0 = u0.data(); d.umap.ptr = up.data(); d.umap.idx = nz(ui); d.umap.val = nzd(uv);
+    d.o0 = D->o0; d.omap = D->omap ? D->omap : zPr.data(); d.ocmap = D->ocmap ? D->ocmap : zPc.data();
+    if (int rc = check_maps(&d)) return rc;
+    dsp_template *T = new dsp_template();
+    struct Guard {
+        dsp_template *t;
+        ~Guard() { if (t) dsp_lp_template_destroy(t); }
+    } guard{T};
+    if (int rc = template_init(T, &d)) return rc;
+    T->kp.w = w; T->kp.nnz = nnz;
+    T->dense_only = true;
+    if (int rc = dense_build(T, A_ptr, A_idx, A_val)) return rc;
+    T->col_perm = col_perm; T->row_perm = row_perm;
+    int *dx = nullptr;
+    if (int rc = upload(col_perm, &dx)) return rc;
+    T->dev_allocs.push_back(dx);
+    T->kp.xperm = dx;                  // rows keep the caller's order: no y permutation
+    guard.t = nullptr;
+    *out = T;
+    return 0;
+}
+
 int dsp_lp_template_set_matrix_params(dsp_template *T, int32_t count, const int32_t *row, const int32_t *col, const int32_t *param,
                                       const double *coef) {
     if (!T || count < 0 || (count > 0 && (!row || !col || !param || !coef))) { g_err = "dsp_lp_template_set_matrix_params: bad arguments"; return DSP_E_ARG; }
+    if (T->dense_only) { g_err = "dsp_lp_template_set_matrix_params: per-problem matrix coefficients are not supported on a dense template"; return DSP_E_ARG; }
     if (T->csr_ptr.empty()) { g_err = "dsp_lp_template_set_matrix_params: the template must come from dsp_lp_template_create_csr"; return DSP_E_ARG; }
     if (T->kp.w != 1 && T->kp.w != 2 && T->kp.w != 4 && T->kp.w != 8 && T->kp.w != 16 && T->kp.w != 32) { g_err = "bad band"; return DSP_E_ARG; }
     KParams &K = T->kp;

@@ -8,6 +8,7 @@ Same names and argument meaning as the reference functions; the only extension i
   record_results(res)                                              wind_battery_LMP.py:272-325
   nuclear_dispatch_optimize(n_time_points, lmps, ...)              nuclear_flowsheet_multiperiod_class.py:72-155
   pv_battery_hydrogen_optimize(n_time_points, input_params, ...)   solar_battery_hydrogen.py:375-606 (design_opt=False)
+  pv_battery_hydrogen_design_optimize(n_time_points, input_params, ...)   the same with design_opt=True (dense kernel)
 
 Where the reference builds a Pyomo MultiPeriodModel and calls SolverFactory("cbc").solve(m) once per signal,
 these build (and cache) one LPTemplate per (flowsheet, T) and hand the whole batch to the CUDA solver.
@@ -21,7 +22,7 @@ import dataclasses
 import numpy as np
 
 from . import templates as TP
-from .solver import BatchLPSolver, OPTIMAL, STATUS_NAMES
+from .solver import KERNEL_DENSE, BatchLPSolver, OPTIMAL, STATUS_NAMES
 
 _SOLVERS = {}
 
@@ -226,10 +227,11 @@ def pv_battery_hydrogen_optimize(n_time_points, input_params, verbose=False, plo
     ``re_h2_parameters`` (solar_battery_hydrogen_inputs.py:79-118).  Returns (design_res, df) like the reference: ``design_res`` with
     the reference's keys (scalars, or arrays [N] for a batch), ``df`` a dict of the operating series [N, T] under the
     reference's column names (one pandas frame per scenario is a ``pd.DataFrame({k: v[i] for k, v in df.items()})`` away).
-    design_opt=True is refused: its six size variables couple every period (not banded within the band kernel's limit)."""
+    design_opt=True is refused here: its six size variables couple every period (not banded within the band kernel's limit);
+    pv_battery_hydrogen_design_optimize solves it on the dense kernel."""
     if input_params.get("design_opt", False):
-        raise NotImplementedError("pv_battery_hydrogen_optimize: design_opt=True is not on the batched GPU path "
-                                  "(six dense size columns); solve the fixed-design LP per candidate size instead")
+        raise NotImplementedError("pv_battery_hydrogen_optimize: design_opt=True is not on the band kernels' path "
+                                  "(six dense size columns); use pv_battery_hydrogen_design_optimize (dense kernel)")
     T = int(n_time_points)
     for k in ("LMP", "pv_resource", "load", "reserve", "pv_mw", "tank_size", "turb_mw"):
         if k not in input_params:
@@ -314,6 +316,105 @@ def pv_battery_hydrogen_optimize(n_time_points, input_params, verbose=False, plo
         "Tank Holdup [kg]": holdup / TP.H2_MOLS_PER_KG, "Excess PV [MW]": (pv_kw[:, None] * cf2 - pv_gen) * 1e-3,
         "Battery Reserve [MW]": ser("battery_reserve", True) * 1e-3, "PEM Reserve [MW]": pem * 1e-3,
         "Turbine Reserve [MW]": ser("turbine_reserve", True) * 1e-3, "Load [MW]": np.broadcast_to(np.atleast_2d(load), (N, T)),
+        "Grid Income [$]": grid_cost, "H2 Revenue [$]": h2_rev, "Operating Cost [$]": pem_var + turb_var,
+    }
+    return design_res, df
+
+
+def pv_battery_hydrogen_design_optimize(n_time_points, input_params, verbose=False):
+    """The reference's PV + battery + PEM + hydrogen tank + turbine case with ``design_opt=True`` (solar_battery_hydrogen.py:375-606,
+    size_constraints :205-236): the added PV, battery power / energy, PEM, tank and turbine sizes are decisions.  Batched over price and
+    load series: ``LMP`` and ``load`` [T] or [N, T]; ``pv_resource`` and ``reserve`` one series (the PV capacity factors multiply the
+    added-PV column, so they are part of the template).  Same ``input_params`` keys as ``re_h2_parameters``; ``pv_mw`` / ``turb_mw``
+    are the existing PV and turbine sizes the design adds to.  Those six columns make A A' dense, so the LPs run on the dense kernel
+    (m <= 1024: T <= 48).  Returns (design_res, df) like the reference, with the optimal sizes per scenario."""
+    T = int(n_time_points)
+    for k in ("LMP", "pv_resource", "load", "reserve"):
+        if k not in input_params:
+            raise KeyError(f"pv_battery_hydrogen_design_optimize: input_params[{k!r}] is required")
+    lmp = np.ascontiguousarray(np.atleast_2d(np.asarray(input_params["LMP"], float))[:, :T])
+    pr = input_params["pv_resource"]
+    if isinstance(pr, dict):
+        cfs = np.array([np.ravel(pr[t]["pv_resource_config"]["capacity_factor"])[0] for t in range(T)], float)
+    else:
+        cfs = np.asarray(pr, float)[..., :T]
+    load = np.atleast_2d(np.asarray(input_params["load"], float))[:, :T]
+    reserve = np.asarray(input_params["reserve"], float)[..., :T]
+    for name, a in (("LMP", lmp), ("pv_resource", cfs), ("load", load), ("reserve", reserve)):
+        if a.shape[-1] != T or (name in ("pv_resource", "reserve") and a.ndim != 1):
+            raise ValueError(f"pv_battery_hydrogen_design_optimize: {name} must provide {T} values per scenario "
+                             f"(pv_resource, reserve: one series), got shape {a.shape}")
+    if np.any(cfs < 0) or not np.all(np.isfinite(cfs)) or not np.all(np.isfinite(load)):
+        raise ValueError("pv_battery_hydrogen_design_optimize: capacity factors must be finite and >= 0, loads finite")
+    N = max(lmp.shape[0], load.shape[0])
+    if lmp.shape[0] not in (1, N) or load.shape[0] not in (1, N):
+        raise ValueError("LMP and load must be one series or one per scenario")
+    par = {k: float(input_params[k]) for k in _SOLAR_COST_KEYS if k in input_params}
+    kw = dict(pv_mw=float(input_params.get("pv_mw", 0.0)), turb_mw=float(input_params.get("turb_mw", 0.0)),
+              max_sales=float(input_params.get("max_sales", 1000.0)), max_purchases=float(input_params.get("max_purchases", 1000.0)))
+    key = ("solar_battery_hydrogen_design", T, tuple(sorted(kw.items())), tuple(sorted(par.items())), cfs.tobytes(), reserve.tobytes())
+    if key not in _SOLVERS:
+        _SOLVERS[key] = BatchLPSolver(TP.solar_battery_hydrogen_design(T, cfs, reserve_mw=reserve, par=par, **kw), kernel=KERNEL_DENSE)
+    sol = _SOLVERS[key]
+    t = sol.t
+    lmp = np.ascontiguousarray(np.broadcast_to(lmp, (N, T)))
+    rp = np.ascontiguousarray(np.broadcast_to(load * 1e3, (N, T)))
+    r = sol.solve_host(lmp, rp, want_x=True)
+    if verbose:
+        print(f"b200ipm (dense kernel): {N} LPs, iterations mean {r.iters.mean():.1f} max {r.iters.max()}, "
+              f"non-optimal {(r.status != OPTIMAL).sum()}")
+    xm = sol.to_model_space(r.x)
+    names = {n: j for j, n in enumerate(t.col_names)}
+    size = {nm: xm[:, names[nm]] for nm in TP.SOLAR_SIZE_COLUMNS}
+
+    def ser(name, blk_level=False):
+        return np.stack([xm[:, names[(f"blk[{k}]." if blk_level else f"blk[{k}].fs.") + name]] for k in range(T)], axis=1)
+    P = dict(TP.SOLAR); P.update(par)
+    k_turb = t.meta["k_turb"]
+    pv_kw = kw["pv_mw"] * 1e3 + size["pv_add_system_capacity"]
+    batt_kw, batt_kwh = size["battery_system_capacity"], size["battery_system_energy"]
+    pem_kw, tank_kg, turb_kw = size["pem_system_capacity"], size["h2_tank_size"], size["turb_system_capacity"]
+    grid, pem = ser("splitter.grid_elec[0]"), ser("pem.electricity[0]")
+    b_in, b_out, soc = ser("battery.elec_in[0]"), ser("battery.elec_out[0]"), ser("battery.state_of_charge[0]")
+    to_turb, to_pipe, holdup = ser("h2_tank.outlet_to_turbine.flow_mol[0]"), ser("h2_tank.outlet_to_pipeline.flow_mol[0]"), ser("h2_tank.tank_holdup[0]")
+    purchase, sales = ser("grid_purchase", True), ser("grid_sales", True)
+    turb_elec = to_turb * k_turb
+    n_weeks = T / 168.0
+    h2_rev = P["h2_price_per_kg"] / TP.H2_MOLS_PER_KG * to_pipe * P["s_per_ts"]
+    grid_cost = lmp * (purchase - sales) * 1e-3
+    pem_var, turb_var = P["pem_var_cost"] * pem, P["turbine_var_cost"] * turb_elec
+    cap_pv, cap_kw, cap_kwh = P["pv_cap_cost"] * size["pv_add_system_capacity"], P["batt_cap_cost_kw"] * batt_kw, P["batt_cap_cost_kwh"] * batt_kwh
+    cap_pem, cap_tank = P["pem_cap_cost"] * pem_kw, P["tank_cap_cost_per_kg"] * tank_kg
+    cap_turb = P["turbine_cap_cost"] * (turb_kw - kw["turb_mw"] * 1e3)
+    fixed = pv_kw * P["pv_op_cost"] + pem_kw * P["pem_op_cost"] + tank_kg * P["tank_op_cost"] + turb_kw * P["turbine_op_cost"]
+    squeeze = (lambda a: float(np.ravel(a)[0])) if N == 1 else (lambda a: np.asarray(a))
+    design_res = {
+        "pv_mw": squeeze(pv_kw * 1e-3), "batt_mw": squeeze(batt_kw * 1e-3), "batt_mwh": squeeze(batt_kwh * 1e-3),
+        "batt_hr": squeeze(np.where(batt_kw > 0, batt_kwh / np.where(batt_kw > 0, batt_kw, 1.0), 0.0)), "pem_mw": squeeze(pem_kw * 1e-3),
+        "tank_tonH2": squeeze(tank_kg * P["kg_to_tons"]), "turb_mw": squeeze(turb_kw * 1e-3),
+        "capital_cost": squeeze(cap_pv + cap_kw + cap_kwh + cap_pem + cap_tank + cap_turb), "capital_cost_pv": squeeze(cap_pv),
+        "capital_cost_batt_kw": squeeze(cap_kw), "capital_cost_batt_kwh": squeeze(cap_kwh), "capital_cost_pem": squeeze(cap_pem),
+        "capital_cost_tank": squeeze(cap_tank), "capital_cost_turb": squeeze(cap_turb),
+        "annual_costs_fixed": squeeze(fixed), "fixed_cost_pv": squeeze(pv_kw * P["pv_op_cost"]), "fixed_cost_pem": squeeze(pem_kw * P["pem_op_cost"]),
+        "fixed_cost_tank": squeeze(tank_kg * P["tank_op_cost"]), "fixed_cost_turb": squeeze(turb_kw * P["turbine_op_cost"]),
+        "annual_costs_variable": squeeze((pem_var + turb_var).sum(1)), "variable_cost_batt": 0.0,
+        "variable_cost_pem": squeeze(pem_var.sum(1)), "variable_cost_turb": squeeze(turb_var.sum(1)),
+        "annual_costs_NG": 0.0, "annual_costs_grid": squeeze(grid_cost.sum(1) * 52 / n_weeks),
+        "annual_costs_total": squeeze((grid_cost + pem_var + turb_var).sum(1) * 52 / n_weeks),
+        "annual_rev_h2": squeeze(h2_rev.sum(1) * 52 / n_weeks), "NPV": squeeze(-r.obj * 1e3), "CO2_lb": 0.0,
+        "status": [STATUS_NAMES[int(v)] for v in r.status], "iters": r.iters,
+    }
+    cf2 = np.broadcast_to(cfs, (N, T))
+    df = {
+        "Total PV Generation [MW]": (grid + pem + b_in) * 1e-3, "Total Power Output [MW]": (grid + b_out + turb_elec) * 1e-3,
+        "PV Power Output [MW]": grid * 1e-3, "PV Power to Battery [MW]": b_in * 1e-3,
+        "State of Charge": soc / np.where(batt_kwh > 0, batt_kwh, 1.0)[:, None], "Battery Power Output [MW]": b_out * 1e-3,
+        "PV Power to PEM [MW]": pem * 1e-3, "PEM H2 Output [kg]": pem * TP.PEM_ELEC_TO_MOL * P["s_per_ts"] / TP.H2_MOLS_PER_KG,
+        "H2 Sales [kg]": to_pipe * P["s_per_ts"] / TP.H2_MOLS_PER_KG, "Turbine H2 Input [kg]": to_turb * P["s_per_ts"] / TP.H2_MOLS_PER_KG,
+        "Turbine Power [MW]": turb_elec * 1e-3, "Purchased Power [MW]": purchase * 1e-3, "Sold Power [MW]": sales * 1e-3,
+        "Tank Holdup [kg]": holdup / TP.H2_MOLS_PER_KG, "Excess PV [MW]": (pv_kw[:, None] * cf2 - (grid + pem + b_in)) * 1e-3,
+        "Battery Reserve [MW]": ser("battery_reserve", True) * 1e-3, "PEM Reserve [MW]": pem * 1e-3,
+        "Turbine Reserve [MW]": ser("turbine_reserve", True) * 1e-3, "Load [MW]": np.broadcast_to(load, (N, T)),
         "Grid Income [$]": grid_cost, "H2 Revenue [$]": h2_rev, "Operating Cost [$]": pem_var + turb_var,
     }
     return design_res, df

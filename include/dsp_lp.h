@@ -27,7 +27,8 @@
  * dispatches_b200/lp_template.py computes all of it.
  *
  * Size limits: half bandwidth of A*A' <= 32 (padded to 1,2,4,8,16,32); any m, n -- the per-LP work region lives in shared
- * memory when it fits (up to ~27 000 doubles) and in a device workspace owned by the template handle otherwise.
+ * memory when it fits (up to ~27 000 doubles) and in a device workspace owned by the template handle otherwise.  A wider LP with
+ * m <= 1024 goes through dsp_lp_template_create_dense (dense normal equations, below).
  *
  * All pointers in dsp_lp_solve_batch are DEVICE pointers, the call is stream-ordered and does not
  * synchronise.  dsp_lp_solve_batch_host takes HOST pointers and does the copies itself.
@@ -75,7 +76,9 @@ typedef struct {
 } dsp_opts;
 
 enum { DSP_KERNEL_AUTO = 0, DSP_KERNEL_BAND = 1, DSP_KERNEL_STAGE = 2 /* generation 2: several LPs per warp */,
-       DSP_KERNEL_STAGE_V1 = 3 /* generation 1: lane per period, T <= 32 (kept as an independent implementation for tests) */ };
+       DSP_KERNEL_STAGE_V1 = 3 /* generation 1: lane per period, T <= 32 (kept as an independent implementation for tests) */,
+       DSP_KERNEL_DENSE = 4 /* dense normal equations, one CTA per LP, m <= 1024: what a dense template runs (AUTO picks it there);
+                               on a band template it replaces the band / stage kernels (a cross-check; no per-problem matrices) */ };
 
 /* Stage descriptor of the wind+battery price-taker flowsheet (wind_battery_LMP.py:172-267, reduced form):
  * any T (T <= 96: on chip, several LPs per warp; longer, up to the reference's full-year 8736 periods of
@@ -149,6 +152,12 @@ int dsp_lp_template_create_csr(const dsp_lp_desc *desc, dsp_template **out);
 int dsp_lp_analyze_csr(const dsp_lp_desc *desc, int32_t *nb, int32_t *w, int32_t *w_natural, int32_t *w_rcm,
                        int32_t *col_perm /*[n] or NULL*/, int32_t *row_perm /*[m] or NULL*/);
 int dsp_lp_template_info(const dsp_template *t, int32_t *m, int32_t *n, int32_t *nb, int32_t *w);
+/* The same hand-over for an LP whose A A' is NOT banded (a design size in a row of every period: solar_battery_hydrogen.py:205-236):
+ * any bandwidth, m <= 1024 (larger: DSP_E_ARG).  dsp_lp_solve_batch then runs the dense kernel (csrc/dsp_dense.cuh): one CTA per LP,
+ * M = A D A' dense, blocked LDL' over 64 x 64 tiles with the trailing updates on the FP64 tensor cores, M in a workspace owned by
+ * the handle.  x / y come back in the caller's order; dsp_lp_template_info reports the true half bandwidth; DSP_KERNEL_BAND / _STAGE
+ * on such a template and dsp_lp_template_set_matrix_params return DSP_E_ARG. */
+int dsp_lp_template_create_dense(const dsp_lp_desc *desc, dsp_template **out);
 /* Per-problem MATRIX coefficients for a template made by dsp_lp_template_create_csr:  A[row][col] = A0[row][col] + sum coef * rparams[param]
  * (row / col in the caller's order; the entry must be in A's pattern).  Needed where a design column is multiplied by per-scenario data --
  * wind system_capacity * capacity_factor[t] with a free wind size, wind_power.py:120-122 + wind_battery_LMP.py:212-216.  The band kernel then
