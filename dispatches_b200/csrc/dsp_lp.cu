@@ -529,7 +529,17 @@ struct DParams {
     double *ws;                        // per-CTA regions: the lower tiles of M, then (vec_in_smem == 0) the per-LP vectors
     long long cta_doubles;
     int vec_in_smem;
+    // per-problem matrix coefficients (dsp_lp_template_create_dense_with_matrix_params): at LP load the CTA derives its LP's CSR
+    // values, CSC values and assembly products at mat_off of its region.  CSR position am_q[u] gets A0 + the sum of
+    // am_coef[k] * rparams[am_param[k]] over k in [am_ptr[u], am_ptr[u+1]) in the caller's term order
+    int nnz, n_amq;
+    long long nterms, mat_off;
+    const int *am_q, *am_ptr, *am_param;
+    const double *am_coef;
+    const int *at_from;                // CSC position -> CSR position
+    const int *asm_qa, *asm_qb;        // assembly product q = A_val[asm_qa[q]] * A_val[asm_qb[q]]
 };
+
 
 // doubles of the per-LP vectors: x z c rd d dx cor rx (n), s wv u ru cors rs (nb), y b rp (m), dy dinv (mp)
 inline long long dense_vec_doubles(int m, int n, int nb, int nt) { return 8LL * n + 6LL * nb + 3LL * m + 2LL * nt * dense::TS; }
@@ -566,7 +576,16 @@ __device__ __forceinline__ double cta_sum(double v, double *red) {
     return r;
 }
 
-template <bool CORR>
+// the matrix values an LP runs with: the template's, or (PerLP) its own at mat_off of the CTA's region (dense_load_matrix).  Read at
+// the point of use, so that the template's instantiation reads its kernel parameters as it always has
+template <bool PerLP>
+__device__ __forceinline__ const double *dense_A(const DWork &W, const DParams &P) { return PerLP ? W.G + P.mat_off : P.A_val; }
+template <bool PerLP>
+__device__ __forceinline__ const double *dense_At(const DWork &W, const DParams &P) { return PerLP ? W.G + P.mat_off + P.nnz : P.At_val; }
+template <bool PerLP>
+__device__ __forceinline__ const double *dense_asm(const DWork &W, const DParams &P) { return PerLP ? W.G + P.mat_off + 2 * P.nnz : P.asm_val; }
+
+template <bool CORR, bool PerLP>
 __device__ void dense_newton(const DWork &W, const DParams &P, double smu, int tid) {
     const int n = P.n, nb = P.nb, m = P.m, mp = P.nt * dense::TS;
     for (int j = tid; j < nb; j += kDenseThreads) {
@@ -586,7 +605,7 @@ __device__ void dense_newton(const DWork &W, const DParams &P, double smu, int t
         double acc = 0.0;
         if (i < m) {
             acc = W.rp[i];
-            for (int q = P.A_ptr[i]; q < P.A_ptr[i + 1]; ++q) acc += P.A_val[q] * W.dx[P.A_idx[q]];
+            for (int q = P.A_ptr[i]; q < P.A_ptr[i + 1]; ++q) acc += dense_A<PerLP>(W, P)[q] * W.dx[P.A_idx[q]];
         }
         W.dy[i] = acc;
     }
@@ -594,7 +613,7 @@ __device__ void dense_newton(const DWork &W, const DParams &P, double smu, int t
     dense::solve(W.G, P.nt, W.dinv, W.dy, tid >> 5, kDenseWarps, tid & 31);
     for (int j = tid; j < n; j += kDenseThreads) {
         double acc = 0.0;
-        for (int q = P.At_ptr[j]; q < P.At_ptr[j + 1]; ++q) acc += P.At_val[q] * W.dy[P.At_idx[q]];
+        for (int q = P.At_ptr[j]; q < P.At_ptr[j + 1]; ++q) acc += dense_At<PerLP>(W, P)[q] * W.dy[P.At_idx[q]];
         W.dx[j] = W.d[j] * acc - W.dx[j];
     }
     __syncthreads();
@@ -621,7 +640,28 @@ __device__ __forceinline__ void dense_step_pass(const DWork &W, const DParams &P
     }
 }
 
+// LP p's own matrix values at mat_off of the CTA's region (per-problem templates), the band kernel's derivation (solve_one) spread over the CTA: CSR values
+// with their terms added in the caller's order, CSC values, assembly products with the host's operands (dense_build).  A non-finite
+// parameter makes non-finite values, and the iteration ends the LP as it ends one with a non-finite price.
+__device__ void dense_load_matrix(const DWork &W, const DParams &P, long long p, int tid) {
+    const double *rp_ = P.rparams + p * P.rstride;
+    double *Av = W.G + P.mat_off, *Atv = Av + P.nnz, *asv = Atv + P.nnz;
+    for (int q = tid; q < P.nnz; q += kDenseThreads) Av[q] = P.A_val[q];
+    __syncthreads();
+    for (int u = tid; u < P.n_amq; u += kDenseThreads) {
+        const int q = P.am_q[u];
+        double acc = Av[q];
+        for (int k = P.am_ptr[u]; k < P.am_ptr[u + 1]; ++k) acc += P.am_coef[k] * rp_[P.am_param[k]];
+        Av[q] = acc;
+    }
+    __syncthreads();
+    for (int q = tid; q < P.nnz; q += kDenseThreads) Atv[q] = Av[P.at_from[q]];
+    for (long long e = tid; e < P.nterms; e += kDenseThreads) asv[e] = Av[P.asm_qa[e]] * Av[P.asm_qb[e]];
+    __syncthreads();
+}
+
 // one attempt on LP p: the band kernel's solve_one (same scaling, start point, proximal term, stopping rule, results rules)
+template <bool PerLP>
 __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, double step_frac, double reg, int it0, int *status_out,
                                 int *iters_out) {
     const int n = P.n, nb = P.nb, m = P.m, nt = P.nt, mp = nt * dense::TS;
@@ -693,7 +733,7 @@ __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, d
         double pmax = 0.0, dmax = 0.0, musum = 0.0, po = 0.0, dobj = 0.0;
         for (int i = tid; i < m; i += kDenseThreads) {
             double acc = W.b[i];
-            for (int q = P.A_ptr[i]; q < P.A_ptr[i + 1]; ++q) acc -= P.A_val[q] * W.x[P.A_idx[q]];
+            for (int q = P.A_ptr[i]; q < P.A_ptr[i + 1]; ++q) acc -= dense_A<PerLP>(W, P)[q] * W.x[P.A_idx[q]];
             W.rp[i] = acc;
             pmax = dmaxd(pmax, fabs(acc));
             dobj += W.b[i] * W.y[i];
@@ -701,7 +741,7 @@ __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, d
         for (int j = tid; j < n; j += kDenseThreads) {
             const double xj = W.x[j], zj = W.z[j];
             double acc = W.c[j] - zj;
-            for (int q = P.At_ptr[j]; q < P.At_ptr[j + 1]; ++q) acc -= P.At_val[q] * W.y[P.At_idx[q]];
+            for (int q = P.At_ptr[j]; q < P.At_ptr[j + 1]; ++q) acc -= dense_At<PerLP>(W, P)[q] * W.y[P.At_idx[q]];
             const double rxj = frcpd(xj);
             double t = zj * rxj + (xj > 1.0 ? reg * rxj * rxj : reg);
             if (j < nb) {
@@ -746,14 +786,14 @@ __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, d
         __syncthreads();
         for (int e = tid; e < P.nent; e += kDenseThreads) {
             double acc = 0.0;
-            for (int q = P.asm_ptr[e]; q < P.asm_ptr[e + 1]; ++q) acc += P.asm_val[q] * W.d[P.asm_col[q]];
+            for (int q = P.asm_ptr[e]; q < P.asm_ptr[e + 1]; ++q) acc += dense_asm<PerLP>(W, P)[q] * W.d[P.asm_col[q]];
             W.G[P.asm_pos[e]] = acc;
         }
         for (int i = m + tid; i < mp; i += kDenseThreads)
             W.G[(long long)dense::tile_index(i / dense::TS, i / dense::TS) * dense::TILE + (i % dense::TS) * (dense::TS + 1)] = 1.0;
         dense::factor(W.G, nt, W.SA, W.SB, W.dinv, warp, kDenseWarps, lane);
         // ---- affine predictor
-        dense_newton<false>(W, P, 0.0, tid);
+        dense_newton<false, PerLP>(W, P, 0.0, tid);
         double ip = 0.0, id = 0.0;
         dense_step_pass<false>(W, P, 0.0, tid, ip, id);
         ip = cta_max(ip, W.red); id = cta_max(id, W.red);
@@ -776,7 +816,7 @@ __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, d
         const double sg = mua / mu;
         const double smu = sg * sg * sg * mu;
         // ---- centring corrector
-        dense_newton<true>(W, P, smu, tid);
+        dense_newton<true, PerLP>(W, P, smu, tid);
         ip = 0.0; id = 0.0;
         dense_step_pass<true>(W, P, smu, tid, ip, id);
         ip = cta_max(ip, W.red); id = cta_max(id, W.red);
@@ -819,6 +859,7 @@ __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, d
     *iters_out = it + it0;
 }
 
+template <bool PerLP>
 __global__ void __launch_bounds__(kDenseThreads, 1) dsp_ipm_dense_kernel(const DParams P) {
     extern __shared__ __align__(16) double dsm[];
     unsigned long long &ticket = *(unsigned long long *)(dsm + kDenseWarps);     // behind the reduction slots
@@ -840,9 +881,10 @@ __global__ void __launch_bounds__(kDenseThreads, 1) dsp_ipm_dense_kernel(const D
         __syncthreads();
         if ((long long)t >= P.N) break;
         int st, it0 = 0;
+        if (PerLP) dense_load_matrix(W, P, (long long)t, threadIdx.x);
         // second attempt (shorter step, stronger proximal term) for the rare LP whose first attempt ends non-optimal
-        dense_solve_one(W, P, (long long)t, P.step_frac, P.reg, 0, &st, &it0);
-        if (st != DSP_OPTIMAL) dense_solve_one(W, P, (long long)t, 0.99, 10.0 * P.reg, it0, &st, &it0);
+        dense_solve_one<PerLP>(W, P, (long long)t, P.step_frac, P.reg, 0, &st, &it0);
+        if (st != DSP_OPTIMAL) dense_solve_one<PerLP>(W, P, (long long)t, 0.99, 10.0 * P.reg, it0, &st, &it0);
     }
 }
 
@@ -1011,6 +1053,11 @@ struct dsp_template {
         int nt, nent;
         const int *A_ptr, *A_idx, *At_ptr, *At_idx, *asm_pos, *asm_ptr, *asm_col;
         const double *A_val, *At_val, *asm_val;
+        // per-problem matrix coefficients (dsp_lp_template_create_dense_with_matrix_params; n_amq == 0: none)
+        int n_amq;
+        long long nterms;
+        const int *am_q, *am_ptr, *am_param, *at_from, *asm_qa, *asm_qb;
+        const double *am_coef;
     };
     mutable Dense dn;
 };
@@ -1139,21 +1186,34 @@ int template_init(dsp_template *T, const dsp_template_desc *D) {
     return 0;
 }
 
+// per-problem matrix terms of a dense template, in the caller's order: CSR position (internal order), rparams index, coefficient
+struct DenseTerms {
+    std::vector<int> q, param;
+    std::vector<double> coef;
+};
+
 // The dense kernel's data for a template whose internal-order CSR is (A_ptr, A_idx, A_val): the CSC, and the assembly list of the
 // lower pattern of A A' in tile-major workspace order -- entry e of M sits at asm_pos[e] and is the sum of
-// asm_val[q] * d[asm_col[q]] over q in [asm_ptr[e], asm_ptr[e+1]).  Host-only analysis, then one upload.
+// asm_val[q] * d[asm_col[q]] over q in [asm_ptr[e], asm_ptr[e+1]).  With per-problem matrix terms (terms non-empty) also what the
+// kernel derives an LP's values from: the terms grouped by CSR position, the CSR position of every CSC entry and the two CSR
+// positions of every assembly product.  Host-only analysis, then one upload.
 constexpr long long kDenseMaxTerms = 1LL << 26;
-int dense_build(dsp_template *T, const std::vector<int> &A_ptr, const std::vector<int> &A_idx, const std::vector<double> &A_val) {
+int dense_build(dsp_template *T, const std::vector<int> &A_ptr, const std::vector<int> &A_idx, const std::vector<double> &A_val,
+                const DenseTerms *terms = nullptr) {
     const int m = T->kp.m, n = T->kp.n, nnz = A_ptr[m];
     const int TS = dense::TS;
-    std::vector<int> At_ptr(n + 1, 0), At_idx(nnz);
+    const bool per_lp = terms && !terms->q.empty();
+    std::vector<int> At_ptr(n + 1, 0), At_idx(nnz), at_from(nnz);
     std::vector<double> At_val(nnz);
     for (int q = 0; q < nnz; ++q) At_ptr[A_idx[q] + 1]++;
     for (int j = 0; j < n; ++j) At_ptr[j + 1] += At_ptr[j];
     {
         std::vector<int> fill(At_ptr.begin(), At_ptr.end() - 1);
         for (int i = 0; i < m; ++i)
-            for (int q = A_ptr[i]; q < A_ptr[i + 1]; ++q) { const int dst = fill[A_idx[q]]++; At_idx[dst] = i; At_val[dst] = A_val[q]; }
+            for (int q = A_ptr[i]; q < A_ptr[i + 1]; ++q) {
+                const int dst = fill[A_idx[q]]++;
+                At_idx[dst] = i; At_val[dst] = A_val[q]; at_from[dst] = q;
+            }
     }
     long long nterms = 0;
     for (int j = 0; j < n; ++j) { const long long c = At_ptr[j + 1] - At_ptr[j]; nterms += c * (c + 1) / 2; }
@@ -1178,8 +1238,9 @@ int dense_build(dsp_template *T, const std::vector<int> &A_ptr, const std::vecto
     for (int e = 0; e < nent; ++e) order[e] = e;
     std::sort(order.begin(), order.end(), [&](int x, int y) { return pos[x] < pos[y]; });
     for (int r = 0; r < nent; ++r) rank[order[r]] = r;
-    std::vector<int> asm_pos(nent), asm_ptr(nent + 1, 0), asm_col((size_t)nterms);
+    std::vector<int> asm_pos(nent), asm_ptr(nent + 1, 0), asm_col((size_t)nterms), asm_qa, asm_qb;
     std::vector<double> asm_val((size_t)nterms);
+    if (per_lp) { asm_qa.resize((size_t)nterms); asm_qb.resize((size_t)nterms); }
     for (int r = 0; r < nent; ++r) { asm_pos[r] = (int)pos[order[r]]; asm_ptr[r + 1] = asm_ptr[r] + cnt[order[r]]; }
     std::vector<int> fill(asm_ptr.begin(), asm_ptr.end() - 1);
     for (int j = 0; j < n; ++j)
@@ -1187,6 +1248,7 @@ int dense_build(dsp_template *T, const std::vector<int> &A_ptr, const std::vecto
             for (int qb = At_ptr[j]; qb <= qa; ++qb) {
                 const int r = rank[slot[(size_t)At_idx[qa] * m + At_idx[qb]]];
                 asm_col[fill[r]] = j;
+                if (per_lp) { asm_qa[fill[r]] = at_from[qa]; asm_qb[fill[r]] = at_from[qb]; }
                 asm_val[fill[r]++] = At_val[qa] * At_val[qb];
             }
     dsp_template::Dense &D = T->dn;
@@ -1205,7 +1267,32 @@ int dense_build(dsp_template *T, const std::vector<int> &A_ptr, const std::vecto
     rc = rc ? rc : ui(asm_col, &D.asm_col);
     rc = rc ? rc : ud(asm_val, &D.asm_val);
     if (rc) return rc;
-    CK(cudaFuncSetAttribute(dsp_ipm_dense_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
+    CK(cudaFuncSetAttribute(dsp_ipm_dense_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
+    if (per_lp) {
+        // the terms grouped by CSR position, each group in the caller's order (the order the band kernel adds them in)
+        const int count = (int)terms->q.size();
+        std::vector<int> by(count);
+        for (int k = 0; k < count; ++k) by[k] = k;
+        std::stable_sort(by.begin(), by.end(), [&](int x, int y) { return terms->q[x] < terms->q[y]; });
+        std::vector<int> am_q, am_ptr(1, 0), am_param(count);
+        std::vector<double> am_coef(count);
+        for (int k = 0; k < count; ++k) {
+            if (k == 0 || terms->q[by[k]] != terms->q[by[k - 1]]) { am_q.push_back(terms->q[by[k]]); am_ptr.push_back(am_ptr.back()); }
+            am_ptr.back()++;
+            am_param[k] = terms->param[by[k]]; am_coef[k] = terms->coef[by[k]];
+        }
+        rc = rc ? rc : ui(am_q, &D.am_q);
+        rc = rc ? rc : ui(am_ptr, &D.am_ptr);
+        rc = rc ? rc : ui(am_param, &D.am_param);
+        rc = rc ? rc : ud(am_coef, &D.am_coef);
+        rc = rc ? rc : ui(at_from, &D.at_from);
+        rc = rc ? rc : ui(asm_qa, &D.asm_qa);
+        rc = rc ? rc : ui(asm_qb, &D.asm_qb);
+        if (rc) return rc;
+        CK(cudaFuncSetAttribute(dsp_ipm_dense_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
+        D.n_amq = (int)am_q.size();
+        D.nterms = nterms;
+    }
     D.nt = (m + TS - 1) / TS;
     D.nent = nent;
     D.ready = true;
@@ -1642,19 +1729,25 @@ static int launch_dense(const dsp_template *T, const KParams &K, cudaStream_t st
     Q.tol = K.tol; Q.feas_tol = K.feas_tol; Q.step_frac = K.step_frac; Q.reg = K.reg; Q.max_iter = K.max_iter;
     Q.obj = K.obj; Q.x_out = K.x_out; Q.y_out = K.y_out; Q.status = K.status; Q.iters = K.iters; Q.ticket = K.ticket;
     Q.xperm = K.xperm; Q.yperm = K.yperm;
+    const bool per_lp = D.n_amq > 0;
+    Q.nnz = K.nnz; Q.n_amq = D.n_amq; Q.nterms = D.nterms;
+    Q.am_q = D.am_q; Q.am_ptr = D.am_ptr; Q.am_param = D.am_param; Q.am_coef = D.am_coef;
+    Q.at_from = D.at_from; Q.asm_qa = D.asm_qa; Q.asm_qb = D.asm_qb;
     const long long vec = dense_vec_doubles(K.m, K.n, K.nb, D.nt);
     Q.vec_in_smem = kDenseSmemFixed + (size_t)vec * 8 <= (size_t)T->smem_optin;
     const size_t smem = kDenseSmemFixed + (Q.vec_in_smem ? (size_t)vec * 8 : 0);
-    Q.cta_doubles = dense::tiles_doubles(D.nt) + (Q.vec_in_smem ? 0 : vec);
+    Q.mat_off = dense::tiles_doubles(D.nt) + (Q.vec_in_smem ? 0 : vec);
+    Q.cta_doubles = Q.mat_off + (per_lp ? 2LL * K.nnz + D.nterms : 0);     // per-problem templates: this LP's A, A' and products
+    void (*kern)(DParams) = per_lp ? dsp_ipm_dense_kernel<true> : dsp_ipm_dense_kernel<false>;
     int occ = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dsp_ipm_dense_kernel, kDenseThreads, smem));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kDenseThreads, smem));
     long long ctas = std::min<long long>(K.N, (long long)T->sm_count * std::max(occ, 1));
     while (ctas > 1 && (size_t)ctas * Q.cta_doubles * 8 > T->ws_cap) ctas /= 2;
     const int rc = grow_ws(T, (size_t)ctas * Q.cta_doubles * 8, st);
     if (rc) return rc;
     Q.ws = T->ws;
     CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
-    dsp_ipm_dense_kernel<<<(unsigned)ctas, kDenseThreads, smem, st>>>(Q);
+    kern<<<(unsigned)ctas, kDenseThreads, smem, st>>>(Q);
     return launched(ctas, kDenseThreads, smem, 1);
 }
 
@@ -2060,16 +2153,19 @@ int dsp_lp_template_create_csr(const dsp_lp_desc *D, dsp_template **out) {
     return 0;
 }
 
-int dsp_lp_template_create_dense(const dsp_lp_desc *D, dsp_template **out) {
-    if (!out) { g_err = "dsp_lp_template_create_dense: out is NULL"; return DSP_E_ARG; }
-    if (!D || D->m <= 0 || D->n <= 0 || !D->A_ptr || !D->A_idx || !D->A_val || !D->u0) { g_err = "dsp_lp_template_create_dense: bad descriptor"; return DSP_E_ARG; }
+// dsp_lp_template_create_dense and its variant with per-problem matrix coefficients (count > 0); fn names the entry point in messages
+static int create_dense(const char *fn, const dsp_lp_desc *D, int32_t count, const int32_t *row, const int32_t *col, const int32_t *param,
+                        const double *coef, dsp_template **out) {
+    const std::string f = fn;
+    if (!out) { g_err = f + ": out is NULL"; return DSP_E_ARG; }
+    if (!D || D->m <= 0 || D->n <= 0 || !D->A_ptr || !D->A_idx || !D->A_val || !D->u0) { g_err = f + ": bad descriptor"; return DSP_E_ARG; }
     if (D->m > kDenseMaxM) {
-        g_err = "dsp_lp_template_create_dense: m = " + std::to_string(D->m) + " rows; the dense kernel takes m <= 1024";
+        g_err = f + ": m = " + std::to_string(D->m) + " rows; the dense kernel takes m <= 1024";
         return DSP_E_ARG;
     }
     const int m = D->m, n = D->n, nnz = D->A_ptr[m];
     for (int q = 0; q < nnz; ++q)
-        if (D->A_idx[q] < 0 || D->A_idx[q] >= n) { g_err = "dsp_lp_template_create_dense: A_idx out of range"; return DSP_E_ARG; }
+        if (D->A_idx[q] < 0 || D->A_idx[q] >= n) { g_err = f + ": A_idx out of range"; return DSP_E_ARG; }
     // internal order: bounded columns first (stable), rows as given (the dense factorisation does not care about bandwidth)
     std::vector<int> col_perm, row_perm(m);
     for (int j = 0; j < n; ++j) if (D->u0[j] < 1e300) col_perm.push_back(j);
@@ -2114,6 +2210,23 @@ int dsp_lp_template_create_dense(const dsp_lp_desc *D, dsp_template **out) {
     d.u0 = u0.data(); d.umap.ptr = up.data(); d.umap.idx = nz(ui); d.umap.val = nzd(uv);
     d.o0 = D->o0; d.omap = D->omap ? D->omap : zPr.data(); d.ocmap = D->ocmap ? D->ocmap : zPc.data();
     if (int rc = check_maps(&d)) return rc;
+    // matrix terms: rows in the caller's order (kept), columns through col_pos, the entry must be in A's pattern
+    if (count < 0 || (count > 0 && (!row || !col || !param || !coef))) { g_err = f + ": bad matrix parameter arguments"; return DSP_E_ARG; }
+    DenseTerms terms;
+    for (int k = 0; k < count; ++k) {
+        if (row[k] < 0 || row[k] >= m || col[k] < 0 || col[k] >= n || param[k] < 0 || param[k] >= D->Pr) {
+            g_err = f + ": matrix parameter " + std::to_string(k) + " index out of range";
+            return DSP_E_ARG;
+        }
+        const int i = row[k], j = col_pos[col[k]];
+        int pos = -1;
+        for (int q = A_ptr[i]; q < A_ptr[i + 1]; ++q) if (A_idx[q] == j) pos = q;
+        if (pos < 0) {
+            g_err = f + ": matrix parameter " + std::to_string(k) + " is on an entry that is not in the sparsity pattern of A (store an explicit nominal value)";
+            return DSP_E_ARG;
+        }
+        terms.q.push_back(pos); terms.param.push_back(param[k]); terms.coef.push_back(coef[k]);
+    }
     dsp_template *T = new dsp_template();
     struct Guard {
         dsp_template *t;
@@ -2122,7 +2235,7 @@ int dsp_lp_template_create_dense(const dsp_lp_desc *D, dsp_template **out) {
     if (int rc = template_init(T, &d)) return rc;
     T->kp.w = w; T->kp.nnz = nnz;
     T->dense_only = true;
-    if (int rc = dense_build(T, A_ptr, A_idx, A_val)) return rc;
+    if (int rc = dense_build(T, A_ptr, A_idx, A_val, &terms)) return rc;
     T->col_perm = col_perm; T->row_perm = row_perm;
     int *dx = nullptr;
     if (int rc = upload(col_perm, &dx)) return rc;
@@ -2131,6 +2244,15 @@ int dsp_lp_template_create_dense(const dsp_lp_desc *D, dsp_template **out) {
     guard.t = nullptr;
     *out = T;
     return 0;
+}
+
+int dsp_lp_template_create_dense(const dsp_lp_desc *D, dsp_template **out) {
+    return create_dense("dsp_lp_template_create_dense", D, 0, nullptr, nullptr, nullptr, nullptr, out);
+}
+
+int dsp_lp_template_create_dense_with_matrix_params(const dsp_lp_desc *D, int32_t count, const int32_t *row, const int32_t *col,
+                                                    const int32_t *param, const double *coef, dsp_template **out) {
+    return create_dense("dsp_lp_template_create_dense_with_matrix_params", D, count, row, col, param, coef, out);
 }
 
 int dsp_lp_template_set_matrix_params(dsp_template *T, int32_t count, const int32_t *row, const int32_t *col, const int32_t *param,

@@ -323,42 +323,54 @@ def pv_battery_hydrogen_optimize(n_time_points, input_params, verbose=False, plo
 
 def pv_battery_hydrogen_design_optimize(n_time_points, input_params, verbose=False):
     """The reference's PV + battery + PEM + hydrogen tank + turbine case with ``design_opt=True`` (solar_battery_hydrogen.py:375-606,
-    size_constraints :205-236): the added PV, battery power / energy, PEM, tank and turbine sizes are decisions.  Batched over price and
-    load series: ``LMP`` and ``load`` [T] or [N, T]; ``pv_resource`` and ``reserve`` one series (the PV capacity factors multiply the
-    added-PV column, so they are part of the template).  Same ``input_params`` keys as ``re_h2_parameters``; ``pv_mw`` / ``turb_mw``
-    are the existing PV and turbine sizes the design adds to.  Those six columns make A A' dense, so the LPs run on the dense kernel
+    size_constraints :205-236): the added PV, battery power / energy, PEM, tank and turbine sizes are decisions.  Batched over price, load,
+    PV and reserve series: ``LMP``, ``load``, ``pv_resource`` and ``reserve`` [T] or [N, T] (``pv_resource`` also as the reference's
+    dict, one series).  With one PV and one reserve series (or N equal rows) the capacity factors are baked into the template; with a
+    series per scenario they are per-problem matrix coefficients of the added-PV column (templates.solar_battery_hydrogen_design(T, None)),
+    and the whole batch still runs in one launch.  Same ``input_params`` keys as ``re_h2_parameters``; ``pv_mw`` / ``turb_mw`` are the
+    existing PV and turbine sizes the design adds to.  The six size columns make A A' dense, so the LPs run on the dense kernel
     (m <= 1024: T <= 48).  Returns (design_res, df) like the reference, with the optimal sizes per scenario."""
     T = int(n_time_points)
     for k in ("LMP", "pv_resource", "load", "reserve"):
         if k not in input_params:
             raise KeyError(f"pv_battery_hydrogen_design_optimize: input_params[{k!r}] is required")
-    lmp = np.ascontiguousarray(np.atleast_2d(np.asarray(input_params["LMP"], float))[:, :T])
+    lmp = np.atleast_2d(np.asarray(input_params["LMP"], float))[:, :T]
     pr = input_params["pv_resource"]
     if isinstance(pr, dict):
         cfs = np.array([np.ravel(pr[t]["pv_resource_config"]["capacity_factor"])[0] for t in range(T)], float)
     else:
         cfs = np.asarray(pr, float)[..., :T]
-    load = np.atleast_2d(np.asarray(input_params["load"], float))[:, :T]
+    load = np.asarray(input_params["load"], float)[..., :T]
     reserve = np.asarray(input_params["reserve"], float)[..., :T]
     for name, a in (("LMP", lmp), ("pv_resource", cfs), ("load", load), ("reserve", reserve)):
-        if a.shape[-1] != T or (name in ("pv_resource", "reserve") and a.ndim != 1):
-            raise ValueError(f"pv_battery_hydrogen_design_optimize: {name} must provide {T} values per scenario "
-                             f"(pv_resource, reserve: one series), got shape {a.shape}")
-    if np.any(cfs < 0) or not np.all(np.isfinite(cfs)) or not np.all(np.isfinite(load)):
-        raise ValueError("pv_battery_hydrogen_design_optimize: capacity factors must be finite and >= 0, loads finite")
-    N = max(lmp.shape[0], load.shape[0])
-    if lmp.shape[0] not in (1, N) or load.shape[0] not in (1, N):
-        raise ValueError("LMP and load must be one series or one per scenario")
+        if a.ndim not in (1, 2) or a.shape[-1] != T:
+            raise ValueError(f"pv_battery_hydrogen_design_optimize: {name} must be [{T}] or [N, {T}], got shape {a.shape}")
+    if np.any(cfs < 0) or not np.all(np.isfinite(cfs)) or not np.all(np.isfinite(load)) or not np.all(np.isfinite(reserve)):
+        raise ValueError("pv_battery_hydrogen_design_optimize: capacity factors must be finite and >= 0, loads and reserves finite")
+    cfs, load, reserve = np.atleast_2d(cfs), np.atleast_2d(load), np.atleast_2d(reserve)
+    N = max(a.shape[0] for a in (lmp, load, cfs, reserve))
+    if any(a.shape[0] not in (1, N) for a in (lmp, load, cfs, reserve)):
+        raise ValueError("LMP, load, pv_resource and reserve must be one series or one per scenario")
     par = {k: float(input_params[k]) for k in _SOLAR_COST_KEYS if k in input_params}
     kw = dict(pv_mw=float(input_params.get("pv_mw", 0.0)), turb_mw=float(input_params.get("turb_mw", 0.0)),
               max_sales=float(input_params.get("max_sales", 1000.0)), max_purchases=float(input_params.get("max_purchases", 1000.0)))
-    key = ("solar_battery_hydrogen_design", T, tuple(sorted(kw.items())), tuple(sorted(par.items())), cfs.tobytes(), reserve.tobytes())
-    if key not in _SOLVERS:
-        _SOLVERS[key] = BatchLPSolver(TP.solar_battery_hydrogen_design(T, cfs, reserve_mw=reserve, par=par, **kw), kernel=KERNEL_DENSE)
+    lmp = np.ascontiguousarray(np.broadcast_to(lmp, (N, T)))
+    if np.all(cfs == cfs[:1]) and np.all(reserve == reserve[:1]):
+        # one PV and one reserve series: baked into the template
+        cf1, rs1 = np.ascontiguousarray(cfs[0]), np.ascontiguousarray(reserve[0])
+        key = ("solar_battery_hydrogen_design", T, tuple(sorted(kw.items())), tuple(sorted(par.items())), cf1.tobytes(), rs1.tobytes())
+        if key not in _SOLVERS:
+            _SOLVERS[key] = BatchLPSolver(TP.solar_battery_hydrogen_design(T, cf1, reserve_mw=rs1, par=par, **kw), kernel=KERNEL_DENSE)
+        rp = np.ascontiguousarray(np.broadcast_to(load * 1e3, (N, T)))
+    else:
+        # a series per scenario: cf_t multiplies the added-PV column -> per-problem matrix coefficients of the dense kernel
+        key = ("solar_battery_hydrogen_design_pvbatched", T, tuple(sorted(kw.items())), tuple(sorted(par.items())))
+        if key not in _SOLVERS:
+            _SOLVERS[key] = BatchLPSolver(TP.solar_battery_hydrogen_design(T, None, par=par, **kw), kernel=KERNEL_DENSE)
+        rp = np.ascontiguousarray(TP.solar_design_rparams(T, np.broadcast_to(load, (N, T)), np.broadcast_to(cfs, (N, T)),
+                                                          np.broadcast_to(reserve, (N, T))))
     sol = _SOLVERS[key]
     t = sol.t
-    lmp = np.ascontiguousarray(np.broadcast_to(lmp, (N, T)))
-    rp = np.ascontiguousarray(np.broadcast_to(load * 1e3, (N, T)))
     r = sol.solve_host(lmp, rp, want_x=True)
     if verbose:
         print(f"b200ipm (dense kernel): {N} LPs, iterations mean {r.iters.mean():.1f} max {r.iters.max()}, "
@@ -404,7 +416,7 @@ def pv_battery_hydrogen_design_optimize(n_time_points, input_params, verbose=Fal
         "annual_rev_h2": squeeze(h2_rev.sum(1) * 52 / n_weeks), "NPV": squeeze(-r.obj * 1e3), "CO2_lb": 0.0,
         "status": [STATUS_NAMES[int(v)] for v in r.status], "iters": r.iters,
     }
-    cf2 = np.broadcast_to(cfs, (N, T))
+    cf2 = np.broadcast_to(cfs, (N, T))                  # each scenario's own PV series
     df = {
         "Total PV Generation [MW]": (grid + pem + b_in) * 1e-3, "Total Power Output [MW]": (grid + b_out + turb_elec) * 1e-3,
         "PV Power Output [MW]": grid * 1e-3, "PV Power to Battery [MW]": b_in * 1e-3,

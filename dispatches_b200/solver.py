@@ -27,7 +27,7 @@ STATUS_NAMES = {OPTIMAL: "optimal", MAX_ITER: "maxIterations", NUMERICAL: "error
 
 KERNEL_AUTO, KERNEL_BAND, KERNEL_STAGE, KERNEL_STAGE_V1, KERNEL_DENSE = 0, 1, 2, 3, 4
 
-EXPORTS = ["dsp_lp_template_create", "dsp_lp_template_set_matrix_params", "dsp_lp_template_set_stage_chain1", "dsp_lp_template_create_csr", "dsp_lp_template_create_dense", "dsp_lp_analyze_csr", "dsp_lp_template_info", "dsp_lp_template_destroy", "dsp_lp_template_set_stage_wb", "dsp_lp_default_opts", "dsp_lp_solve_batch",
+EXPORTS = ["dsp_lp_template_create", "dsp_lp_template_set_matrix_params", "dsp_lp_template_set_stage_chain1", "dsp_lp_template_create_csr", "dsp_lp_template_create_dense", "dsp_lp_template_create_dense_with_matrix_params", "dsp_lp_analyze_csr", "dsp_lp_template_info", "dsp_lp_template_destroy", "dsp_lp_template_set_stage_wb", "dsp_lp_default_opts", "dsp_lp_solve_batch",
            "dsp_lp_solve_batch_host", "dsp_lp_launch_count", "dsp_lp_last_launch", "dsp_lp_last_error",
            "dsp_lp_version", "dsp_lp_fp64_peak_tflops"]
 
@@ -88,6 +88,8 @@ def load_library():
     lib.dsp_lp_template_create_csr.restype = C.c_int
     lib.dsp_lp_template_create_dense.argtypes = [C.POINTER(_LpDesc), C.POINTER(C.c_void_p)]
     lib.dsp_lp_template_create_dense.restype = C.c_int
+    lib.dsp_lp_template_create_dense_with_matrix_params.argtypes = [C.POINTER(_LpDesc), C.c_int32] + [C.c_void_p] * 4 + [C.POINTER(C.c_void_p)]
+    lib.dsp_lp_template_create_dense_with_matrix_params.restype = C.c_int
     lib.dsp_lp_analyze_csr.argtypes = [C.POINTER(_LpDesc)] + [C.POINTER(C.c_int32)] * 4 + [C.c_void_p, C.c_void_p]
     lib.dsp_lp_analyze_csr.restype = C.c_int
     lib.dsp_lp_template_set_matrix_params.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -165,8 +167,6 @@ class BatchLPSolver:
         # a template whose A A' is wider than the band kernels take runs on the dense kernel: the library gets the plain LP
         self.dense = kernel == KERNEL_DENSE and t.w > 32
         if self.dense:
-            if t.amap is not None:
-                raise ValueError("the dense kernel does not take per-problem matrix coefficients")
             native_setup = True
         A = t.A.tocsr(); A.sort_indices()
         Cm = t.Cmap.tocsr(); Bm = t.Bmap.tocsr()
@@ -185,8 +185,15 @@ class BatchLPSolver:
                         b0=p("b0"), bmap=_ParamMap(p("bm_ptr"), p("bm_idx"), p("bm_val")),
                         u0=p("u0"), umap=_ParamMap(p("um_ptr"), p("um_idx"), p("um_val")),
                         o0=float(t.o0), omap=p("omap"), ocmap=p("ocmap"))
-            create = "dsp_lp_template_create_dense" if self.dense else "dsp_lp_template_create_csr"
-            rc = getattr(self.lib, create)(C.byref(d), C.byref(h))
+            if self.dense and t.amap is not None:         # per-problem matrix coefficients of a dense template come with its creation
+                create = "dsp_lp_template_create_dense_with_matrix_params"
+                am = [_i32(t.amap[0]), _i32(t.amap[1]), _i32(t.amap[2]), _f64(t.amap[3])]
+                keep.update(am=am)
+                rc = self.lib.dsp_lp_template_create_dense_with_matrix_params(C.byref(d), len(am[0]), *(a.ctypes.data_as(C.c_void_p) for a in am),
+                                                                              C.byref(h))
+            else:
+                create = "dsp_lp_template_create_dense" if self.dense else "dsp_lp_template_create_csr"
+                rc = getattr(self.lib, create)(C.byref(d), C.byref(h))
             if rc != 0:
                 raise RuntimeError(f"{create} failed ({rc}): {self.lib.dsp_lp_last_error().decode()}")
         else:
@@ -210,7 +217,7 @@ class BatchLPSolver:
             if rc != 0:
                 raise RuntimeError(f"dsp_lp_template_create failed ({rc}): {self.lib.dsp_lp_last_error().decode()}")
         self.handle = h
-        if t.amap is not None:
+        if t.amap is not None and not self.dense:
             ar, ac, ak, av = _i32(t.amap[0]), _i32(t.amap[1]), _i32(t.amap[2]), _f64(t.amap[3])
             vp_ = lambda a: a.ctypes.data_as(C.c_void_p)
             rc = self.lib.dsp_lp_template_set_matrix_params(h, len(ar), vp_(ar), vp_(ac), vp_(ak), vp_(av))

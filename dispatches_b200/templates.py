@@ -508,7 +508,10 @@ SOLAR_SIZE_COLUMNS = ("pv_add_system_capacity", "battery_system_capacity", "batt
                       "h2_tank_size", "turb_system_capacity")
 
 
-def solar_battery_hydrogen_design(T: int, pv_cfs, pv_mw=0.0, turb_mw=0.0, reserve_mw=100.0, max_sales=1000.0, max_purchases=1000.0,
+PV_CF_NOMINAL = 0.5    # nominal capacity factor of the per-problem PV entries: a power of two, so -(0.5 + (cf - 0.5)) is -cf exactly on a dyadic grid
+
+
+def solar_battery_hydrogen_design(T: int, pv_cfs=None, pv_mw=0.0, turb_mw=0.0, reserve_mw=100.0, max_sales=1000.0, max_purchases=1000.0,
                                   par=None) -> LPTemplate:
     """pv_battery_hydrogen_optimize with design_opt=True (size_constraints, solar_battery_hydrogen.py:205-236): the six sizes
     (added PV, battery power / energy, PEM, tank, turbine) are columns of their own, each in a ``<=`` row of every period.  Those six
@@ -516,6 +519,13 @@ def solar_battery_hydrogen_design(T: int, pv_cfs, pv_mw=0.0, turb_mw=0.0, reserv
     ``lp_template.find_linking_columns`` finds exactly these six, and without them the half bandwidth is 31 (DESIGN §2 row (f)).
     The PV capacity factors multiply the added-PV column, so the PV series is part of the template; the batch runs over
     cparams = lmp[T] and rparams = load_kw[T].
+
+    ``pv_cfs=None``: a PV and a reserve series per problem.  cf_t becomes a per-problem matrix coefficient of pv_add_system_capacity in
+    pv_max[t] and min_reserve[t] for every t (zero hours included: the entry stays in the pattern), the reserve and cf_t * pv_mw go into
+    the right-hand sides, and ``reserve_mw`` is not read.  rparams = [load_kw (T) | cf_t - PV_CF_NOMINAL (T) | reserve_kw (T)], where
+    reserve_kw[t] is the reserve the reference asks of period t (:347-348: the series' previous hour, hour 0 for t = 0;
+    ``solar_design_rparams`` builds the rows).  The entry is -(PV_CF_NOMINAL + rparams[T + t]), equal to -cf_t exactly for capacity
+    factors on a dyadic grid, so such an LP is the baked template's LP bit for bit when pv_mw = 0.
 
     Presolve against the raw LP: arcs substituted as in ``solar_battery_hydrogen``; the per-period nameplate power / energy and PV
     capacity copies replaced by the size columns they are bounded by (nothing else prices them, so they sit at the size); the
@@ -525,15 +535,18 @@ def solar_battery_hydrogen_design(T: int, pv_cfs, pv_mw=0.0, turb_mw=0.0, reserv
     and next to kW-scale flows they would set the scale of the whole LP; the cyclic chain of nameplate-power links (:47, :61) is gone with
     the copies, so none of its redundant links remains; grid_sales - grid_purchase <= max_sales is implied by the bounds."""
     P = dict(SOLAR); P.update(par or {})
-    cf = np.asarray(pv_cfs, float).reshape(T)
-    reserve = np.broadcast_to(np.asarray(reserve_mw, float), (T,))
+    per_problem = pv_cfs is None
+    if not per_problem:
+        cf = np.asarray(pv_cfs, float).reshape(T)
+        reserve = np.broadcast_to(np.asarray(reserve_mw, float), (T,))
     pv_base, turb_base = pv_mw * 1e3, turb_mw * 1e3
     k_turb = P["s_per_ts"] / H2_MOLS_PER_KG * P["h2_turb_conv"]
     k_res = P["h2_turb_conv"] / H2_MOLS_PER_KG
     k_pem = P["s_per_ts"] * PEM_ELEC_TO_MOL
     ramp = P["turbine_ramp_mw_per_min"] * 1e3
     fmax = P["flow_mol_ub"]
-    B = TemplateBuilder(f"solar_battery_hydrogen_design_T{T}", Pc=T, Pr=T)
+    iC, iR = T, 2 * T                                       # per-problem mode: rparams offsets of the cf terms and the reserves
+    B = TemplateBuilder(f"solar_battery_hydrogen_design_T{T}" + ("_pvbatched" if per_problem else ""), Pc=T, Pr=3 * T if per_problem else T)
     ann = 52.143 / (T / 168.0)
     kk = 1e-3 * PA * ann
     Va = B.var("pv_add_system_capacity")
@@ -570,7 +583,12 @@ def solar_battery_hydrogen_design(T: int, pv_cfs, pv_mw=0.0, turb_mw=0.0, reserv
     for t in range(T):
         tm = (t - 1) % T
         pv = {g[t]: 1.0, pe[t]: 1.0, i[t]: 1.0}                       # pv.electricity = grid + PEM + battery (elec_splitter.py:115-117)
-        B.le(f"pv_max[{t}]", {**pv, Va: -cf[t]} if cf[t] != 0.0 else pv, cf[t] * pv_base)                      # solar_pv.py:82-84
+        if per_problem:                                               # -cf_t Va <= ... and cf_t pv_base with cf_t = nominal + rparams
+            a_cf = (-PV_CF_NOMINAL, {iC + t: -1.0})
+            b_cf = (PV_CF_NOMINAL * pv_base, {iC + t: pv_base} if pv_base != 0.0 else {})
+            B.le(f"pv_max[{t}]", {**pv, Va: a_cf}, b_cf)
+        else:
+            B.le(f"pv_max[{t}]", {**pv, Va: -cf[t]} if cf[t] != 0.0 else pv, cf[t] * pv_base)                  # solar_pv.py:82-84
         row = {s[t]: 1.0, i[t]: -ETA_C, o[t]: 1.0 / ETA_D}
         row[s[tm]] = row.get(s[tm], 0.0) - 1.0
         B.eq(f"soc[{t}]", row)
@@ -587,21 +605,39 @@ def solar_battery_hydrogen_design(T: int, pv_cfs, pv_mw=0.0, turb_mw=0.0, reserv
         B.eq(f"meet_load[{t}]", {g[t]: 1.0, o[t]: 1.0, tt[t]: k_turb, gp[t]: 1.0, gs[t]: -1.0}, (0.0, {t: 1.0}))
         B.le(f"turbine_reserve_lb1[{t}]", {tr[t]: 1.0, hd[t]: -k_res})
         B.le(f"turbine_reserve_lb2[{t}]", {tr[t]: 1.0, tt[t]: k_turb, Tc: -1.0})
-        r1 = (max(reserve[max(t - 1, 0):t]) if t > 0 else reserve[0]) * 1e3
         row = {br[t]: -1.0, tr[t]: -1.0, g[t]: 1.0, i[t]: 1.0}                       # PV headroom C cf - w with w substituted
-        if cf[t] != 0.0:
-            row[Va] = -cf[t]
-        B.le(f"min_reserve[{t}]", row, -r1 + cf[t] * pv_base)
+        if per_problem:
+            row[Va] = a_cf
+            B.le(f"min_reserve[{t}]", row, (b_cf[0], {**b_cf[1], iR + t: -1.0}))
+        else:
+            r1 = (max(reserve[max(t - 1, 0):t]) if t > 0 else reserve[0]) * 1e3
+            if cf[t] != 0.0:
+                row[Va] = -cf[t]
+            B.le(f"min_reserve[{t}]", row, -r1 + cf[t] * pv_base)
         if T > 1:                                                                            # both ramp rows (:323-324) as one ranged row
             rr = B.var(f"ramp_range[{t}]", ub=2.0 * ramp)
             B.eq(f"energy_ramp[{t}]", {tt[t]: k_turb, tt[tm]: -k_turb, rr: 1.0}, ramp)
     B.le("battery_min_duration", {Bc: 0.5, Be: -1.0})                                        # :234-235
     B.le("battery_max_duration", {Be: 1.0, Bc: -8.0})
     B.le("capacity_requirement", {Bc: -P["capacity_credit_battery"], Tc: -1.0}, -P["capacity_requirement"] * 1e3)
-    B.meta.update(kind="solar_battery_hydrogen_design", T=T, ann=ann, k_turb=k_turb, pv_base=pv_base, turb_base=turb_base, pv_cfs=cf.copy())
+    B.meta.update(kind="solar_battery_hydrogen_design", T=T, ann=ann, k_turb=k_turb, pv_base=pv_base, turb_base=turb_base,
+                  pv_cfs=None if per_problem else cf.copy(), per_problem_pv=per_problem)
     # not equilibrated: the six size columns sit in rows of every period, and the geometric-mean row / column scaling then stretches
     # the bounds and costs over 1e-8 .. 1e11 (the interior-point iterates diverge); in kW, mol and $ the LP solves in about 22 iterations
     return B.build(equilibrate=False)
+
+
+def solar_design_rparams(T, load_mw, pv_cfs, reserve_mw):
+    """rparams rows of solar_battery_hydrogen_design(T, None): [load_kw (T) | cf_t - PV_CF_NOMINAL (T) | reserve_kw (T)] with
+    reserve_kw[t] = reserve of hour t - 1 (hour 0 for t = 0) in kW (solar_battery_hydrogen.py:347-348); each argument [T] or [N, T]"""
+    ld, cf, rs = (np.atleast_2d(np.asarray(a, float)) for a in (load_mw, pv_cfs, reserve_mw))
+    N = max(ld.shape[0], cf.shape[0], rs.shape[0])
+    out = np.empty((N, 3 * T))
+    out[:, :T] = ld * 1e3
+    out[:, T:2 * T] = cf - PV_CF_NOMINAL
+    out[:, 2 * T] = rs[:, 0] * 1e3
+    out[:, 2 * T + 1:] = rs[:, :T - 1] * 1e3
+    return out
 
 
 def solar_rparams(T, pv_cfs, pv_mw, load_mw):

@@ -156,8 +156,17 @@ int dsp_lp_template_info(const dsp_template *t, int32_t *m, int32_t *n, int32_t 
  * any bandwidth, m <= 1024 (larger: DSP_E_ARG).  dsp_lp_solve_batch then runs the dense kernel (csrc/dsp_dense.cuh): one CTA per LP,
  * M = A D A' dense, blocked LDL' over 64 x 64 tiles with the trailing updates on the FP64 tensor cores, M in a workspace owned by
  * the handle.  x / y come back in the caller's order; dsp_lp_template_info reports the true half bandwidth; DSP_KERNEL_BAND / _STAGE
- * on such a template and dsp_lp_template_set_matrix_params return DSP_E_ARG. */
+ * on such a template and dsp_lp_template_set_matrix_params return DSP_E_ARG (per-problem matrix coefficients of a dense template are
+ * given at creation, below). */
 int dsp_lp_template_create_dense(const dsp_lp_desc *desc, dsp_template **out);
+/* The same with per-problem MATRIX coefficients, given at creation:  A[row][col] = A0[row][col] + sum coef * rparams[param], the terms of
+ * one entry added in the order given (the semantics of dsp_lp_template_set_matrix_params; row / col in the caller's order).  Needed where
+ * a design column is multiplied by per-scenario data -- the added-PV size times the capacity factor of every hour with a PV series per
+ * scenario, solar_pv.py:82-84 + solar_battery_hydrogen.py:205-236.  An entry outside A's pattern or an index out of range is DSP_E_ARG;
+ * count == 0 is dsp_lp_template_create_dense.  At LP load the dense kernel derives the LP's CSR and CSC values and the products of its
+ * assembly list into the LP's workspace region (2 nnz + the assembly list's length more doubles per LP in flight). */
+int dsp_lp_template_create_dense_with_matrix_params(const dsp_lp_desc *desc, int32_t count, const int32_t *row, const int32_t *col,
+                                                    const int32_t *param, const double *coef, dsp_template **out);
 /* Per-problem MATRIX coefficients for a template made by dsp_lp_template_create_csr:  A[row][col] = A0[row][col] + sum coef * rparams[param]
  * (row / col in the caller's order; the entry must be in A's pattern).  Needed where a design column is multiplied by per-scenario data --
  * wind system_capacity * capacity_factor[t] with a free wind size, wind_power.py:120-122 + wind_battery_LMP.py:212-216.  The band kernel then
