@@ -8,8 +8,12 @@ slacks are basic, which columns sit at 0 or at u), re-solves B x_B = b - N x_N a
 verifies the KKT conditions exactly.  A basic row slack is a unit column whose value must come out exactly 0 (the rows are
 equalities) and whose reduced cost forces y_i = 0.  Taking the basis from HiGHS rather than guessing it from x is what certifies
 degenerate vertices: the dispatch LPs have zero prices, idle empty batteries and zero capacity factors, so fewer than m columns lie
-strictly inside their bounds at almost every optimum.  The answer is the optimum of that very LP, not another solver's
-approximation of it; when the basis does not verify, it raises (there is no fall-back to the floating-point answer).  The optimum
+strictly inside their bounds at almost every optimum.  A degenerate vertex is certified from HiGHS' basis or from an exact repair of
+it: HiGHS solves in floating point (and drops entries below its small-matrix-value threshold, such as the 1.2e-16 of sin(pi) in a
+PV series), so its basis can be primal infeasible in exact arithmetic by 1e-14 or so; a bounded dual simplex in exact arithmetic
+(_repair) then pivots it to a basis that verifies.  Everything is verified against the LP as the kernels receive it, tiny entries
+included.  The answer is the optimum of that very LP, not another solver's approximation of it; when the basis does not verify, it
+raises (there is no fall-back to the floating-point answer).  The optimum
 is unique in x when every nonbasic reduced cost is nonzero, and unique in y when every basic column lies strictly inside its bounds
 (and no row slack is basic).  Either way, ``fixed`` marks the columns every optimal x has at the bound x* sits at (r*_j != 0,
 complementary slackness with y*) and ``inside`` the columns at which every optimal y has a zero reduced cost (0 < x*_j < u_j).
@@ -46,6 +50,7 @@ class ExactOptimum:
     r: np.ndarray = None       # [n] r* = c - A'y*, rounded from the exact value
     fixed: np.ndarray = None   # [n] bool, r*_j != 0: every optimal x has x_j at the bound x*_j sits at
     inside: np.ndarray = None  # [n] bool, 0 < x*_j < u_j: every optimal y has r_j(y) = 0
+    pivots: int = 0            # dual simplex pivots that repaired HiGHS' basis (0: it verified as it is)
 
 
 def _fr(v):
@@ -113,7 +118,9 @@ def _objective_constant(t, cp, rp):
 def highs_basis(c, A, b, u):
     """HiGHS simplex (tolerances oracle.highs.TIGHT) on  min c'x  s.t.  A x = b, 0 <= x <= u  (A scipy CSC): its final basis as
     (col [n] int8: 0 at 0, 1 basic, 2 at u;  row_basic [m] bool: the row's slack is basic).  scipy's linprog returns x but not
-    the basis, so this reads it through scipy's bundled HiGHS binding, which is private: it fails loudly where that is missing."""
+    the basis, so this reads it through scipy's bundled HiGHS binding, which is private: it fails loudly where that is missing.
+    passModel may warn (it drops entries below 1e-9 in magnitude): the basis is still taken, and exact_optimum verifies it -- or its
+    repair -- against the full LP.  An error, of passModel or of the solve, raises."""
     from scipy.optimize._highspy import _core as hc
     m, n = A.shape
     lp = hc.HighsLp()
@@ -129,7 +136,7 @@ def highs_basis(c, A, b, u):
     h = hc._Highs()
     for k, v in dict(output_flag=False, solver="simplex", simplex_strategy=1, **TIGHT).items():      # (1: dual simplex)
         h.setOptionValue(k, v)
-    if h.passModel(lp) != hc.HighsStatus.kOk or h.run() != hc.HighsStatus.kOk:
+    if h.passModel(lp) not in (hc.HighsStatus.kOk, hc.HighsStatus.kWarning) or h.run() != hc.HighsStatus.kOk:
         raise NotCertified("HiGHS failed")
     if h.getModelStatus() != hc.HighsModelStatus.kOptimal:
         raise NotCertified(f"HiGHS: {h.modelStatusToString(h.getModelStatus())}")
@@ -143,36 +150,17 @@ def highs_basis(c, A, b, u):
     return col, np.array([v == hc.HighsBasisStatus.kBasic for v in bs.row_status])
 
 
-def exact_optimum(t, cparams_row, rparams_row, basis=None) -> ExactOptimum:
-    """the exact optimum of one LP of template t (see the module docstring); raises NotCertified when HiGHS' final basis -- or
-    ``basis``, a (col, row_basic) pair as highs_basis returns it -- does not verify in exact arithmetic"""
-    cp = np.asarray(cparams_row, float)
-    rp = np.asarray(rparams_row if rparams_row is not None else np.zeros(0), float)
-    c, b, u, _ = t.instantiate(cp, rp)
-    A = t.matrix(rp).tocsc(copy=True)
-    A.sort_indices()
-    m, n = A.shape
-    fin = np.isfinite(u)
-    col, row_basic = highs_basis(c, A, b, u) if basis is None else basis
-    basic, at_hi = col == 1, col == 2
-    at_lo = col == 0
-    if (at_hi & ~fin).any():
-        raise NotCertified("an unbounded column at its upper bound")
-    if basic.sum() + row_basic.sum() != m:
-        raise NotCertified(f"{int(basic.sum())} basic columns and {int(row_basic.sum())} basic row slacks for {m} rows")
-    # exact data
-    cF, bF = _fr(c), _fr(b)
-    uF = [Fraction(float(v)) if f else None for v, f in zip(u, fin)]
-    cols = [(A.indices[A.indptr[j]:A.indptr[j + 1]], _fr(A.data[A.indptr[j]:A.indptr[j + 1]])) for j in range(n)]
+def _vertex(cols, cF, bF, uF, col, row_basic):
+    """the basic solution of the basis (col, row_basic) in exact arithmetic: x [n], the values of the basic row slacks {row: s_i},
+    y [m] and r = c - A'y [n]"""
+    m, n = len(bF), len(cF)
+    bidx, sidx = np.flatnonzero(col == 1), np.flatnonzero(row_basic)
     xF = [Fraction(0)] * n
-    for j in np.flatnonzero(at_hi):
-        xF[j] = uF[j]
     rhs = list(bF)
-    for j in np.flatnonzero(at_hi):
+    for j in np.flatnonzero(col == 2):
+        xF[j] = uF[j]
         for i, a in zip(*cols[j]):
             rhs[i] -= a * xF[j]
-    bidx = np.flatnonzero(basic)
-    sidx = np.flatnonzero(row_basic)
     pos = {j: k for k, j in enumerate(bidx)}
     rowsB = [dict() for _ in range(m)]                 # B x_B = rhs: equation i, variable pos[j]; then the basic row slacks
     for j in bidx:
@@ -183,17 +171,127 @@ def exact_optimum(t, cparams_row, rparams_row, basis=None) -> ExactOptimum:
     xB = _solve_sparse(rowsB, rhs, m)
     for j, v in zip(bidx, xB):
         xF[j] = v
-    if any(xB[len(bidx):]):
-        raise NotCertified("a basic row slack is nonzero")
-    rowsT = [{int(i): a for i, a in zip(*cols[j])} for j in bidx] + [{int(i): Fraction(1)} for i in sidx]   # B'y = c_B
-    yF = _solve_sparse(rowsT, [cF[j] for j in bidx] + [Fraction(0)] * len(sidx), m)
-    # exact KKT
+    yF = _solve_sparse(_basis_rows(cols, bidx, sidx), [cF[j] for j in bidx] + [Fraction(0)] * len(sidx), m)   # B'y = c_B
     rF = []
     for j in range(n):
         s = cF[j]
         for i, a in zip(*cols[j]):
             s -= a * yF[i]
         rF.append(s)
+    return xF, dict(zip((int(i) for i in sidx), xB[len(bidx):])), yF, rF
+
+
+def _basis_rows(cols, bidx, sidx):
+    """the rows of B': one per basic column, then one per basic row slack (a unit column)"""
+    return [{int(i): a for i, a in zip(*cols[j])} for j in bidx] + [{int(i): Fraction(1)} for i in sidx]
+
+
+def _primal_violations(xF, sF, col, uF):
+    """{variable: signed violation} of the basic variables outside their bounds (column j, or row slack i as variable n + i, whose
+    bounds are [0, 0]): > 0 above the upper bound, < 0 below 0"""
+    n = len(xF)
+    out = {}
+    for j in np.flatnonzero(col == 1):
+        if xF[j] < 0:
+            out[int(j)] = xF[j]
+        elif uF[j] is not None and xF[j] > uF[j]:
+            out[int(j)] = xF[j] - uF[j]
+    out.update({n + i: v for i, v in sF.items() if v})
+    return out
+
+
+MAX_PIVOTS = 64          # the repair's pivot limit (the 48-hour design LPs need up to 48: one pivot per row left off by HiGHS)
+REPAIR_GATE = 1e-8       # the repair starts only where every exact infeasibility is at most this, relative to the primal scale
+
+
+def _repair(cols, cF, bF, uF, col, row_basic, vertex, scale):
+    """a bounded dual simplex in exact arithmetic from a dual feasible basis that is primal infeasible by at most REPAIR_GATE of the
+    primal scale (HiGHS' basis of an LP whose floating-point solve dropped a tiny entry, or whose rounding hid a 1e-14 infeasibility).
+    Row slack i is a column e_i with bounds [0, 0]; a nonbasic column with u_j = 0 is fixed (never enters, either sign of r_j).
+    Leaving: the most infeasible basic variable (lowest index on ties).  Entering: the ratio test |r_j / alpha_j| over the nonbasic
+    columns that move it towards its bound, Bland's rule (lowest index) on ties.  After each pivot the basic solution is solved
+    again from scratch.  A basis that is also dual infeasible is not repaired (the LPs here never need a primal simplex leg): it
+    raises, as does a ratio test with no candidate (the LP is infeasible in exact arithmetic) or MAX_PIVOTS pivots without a
+    feasible basis.  Returns (col, row_basic, vertex, pivots)."""
+    m, n = len(bF), len(cF)
+    col, row_basic = col.copy(), row_basic.copy()
+    fixed = np.array([u is not None and u == 0 for u in uF])
+    for pivots in range(MAX_PIVOTS + 1):
+        xF, sF, yF, rF = vertex
+        viol = _primal_violations(xF, sF, col, uF)
+        if not viol:
+            return col, row_basic, vertex, pivots
+        if pivots == 0:
+            worst = max(abs(v) for v in viol.values())
+            if worst > Fraction(REPAIR_GATE) * Fraction(scale):
+                raise NotCertified(f"HiGHS' basis is primal infeasible by {float(worst / Fraction(scale)):.1e} of the primal scale, "
+                                   f"too far to repair")
+            if any(not fixed[j] and ((col[j] == 0 and rF[j] < 0) or (col[j] == 2 and rF[j] > 0)) for j in range(n)):
+                raise NotCertified("HiGHS' basis is primal and dual infeasible")
+        elif pivots == MAX_PIVOTS:
+            break
+        p = min(viol, key=lambda v: (-abs(viol[v]), v))
+        bidx, sidx = np.flatnonzero(col == 1), np.flatnonzero(row_basic)
+        k = int(np.searchsorted(bidx, p)) if p < n else len(bidx) + int(np.searchsorted(sidx, p - n))
+        e = [Fraction(0)] * m
+        e[k] = Fraction(1)
+        rho = _solve_sparse(_basis_rows(cols, bidx, sidx), e, m)          # row k of B^-1: x_p = beta_p - sum_j alpha_j x_j
+        up = viol[p] < 0                                                  # x_p must increase
+        best = None
+        for j in range(n):
+            if col[j] == 1 or fixed[j]:
+                continue
+            alpha = sum((a * rho[i] for i, a in zip(*cols[j]) if rho[i]), Fraction(0))
+            if alpha == 0 or (alpha < 0) != ((col[j] == 0) == up):
+                continue
+            ratio = abs(rF[j] / alpha)
+            if best is None or ratio < best[0]:
+                best = (ratio, j)
+        if best is None:
+            raise NotCertified("the repair's ratio test found no entering column: the LP is infeasible in exact arithmetic")
+        col[best[1]] = 1
+        if p < n:
+            col[p] = 0 if up else 2
+        else:
+            row_basic[p - n] = False
+        vertex = _vertex(cols, cF, bF, uF, col, row_basic)
+    raise NotCertified(f"HiGHS' basis not repaired in {MAX_PIVOTS} pivots")
+
+
+def exact_optimum(t, cparams_row, rparams_row, basis=None) -> ExactOptimum:
+    """the exact optimum of one LP of template t (see the module docstring); raises NotCertified when HiGHS' final basis -- repaired
+    by _repair where it is off by exact primal infeasibility alone -- or ``basis``, a (col, row_basic) pair as highs_basis returns
+    it and verified as it is, does not verify in exact arithmetic"""
+    cp = np.asarray(cparams_row, float)
+    rp = np.asarray(rparams_row if rparams_row is not None else np.zeros(0), float)
+    c, b, u, _ = t.instantiate(cp, rp)
+    A = t.matrix(rp).tocsc(copy=True)
+    A.sort_indices()
+    m, n = A.shape
+    fin = np.isfinite(u)
+    col, row_basic = highs_basis(c, A, b, u) if basis is None else basis
+    if (col == 2)[~fin].any():
+        raise NotCertified("an unbounded column at its upper bound")
+    if (col == 1).sum() + row_basic.sum() != m:
+        raise NotCertified(f"{int((col == 1).sum())} basic columns and {int(row_basic.sum())} basic row slacks for {m} rows")
+    # exact data
+    cF, bF = _fr(c), _fr(b)
+    uF = [Fraction(float(v)) if f else None for v, f in zip(u, fin)]
+    cols = [(A.indices[A.indptr[j]:A.indptr[j + 1]], _fr(A.data[A.indptr[j]:A.indptr[j + 1]])) for j in range(n)]
+    vertex = _vertex(cols, cF, bF, uF, col, row_basic)
+    pivots = 0
+    if basis is None:
+        scale = max(1.0, float(np.abs(b).max(initial=0.0)), float(np.abs(u[fin]).max(initial=0.0)))
+        col, row_basic, vertex, pivots = _repair(cols, cF, bF, uF, col, row_basic, vertex, scale)
+    xF, sF, yF, rF = vertex
+    if pivots:                                         # a fixed column left at 0 by the repair sits at the bound its r_j asks for
+        zero_u = np.array([v is not None and v == 0 for v in uF])
+        col = np.where((col == 0) & zero_u & np.array([v < 0 for v in rF]), 2, col).astype(np.int8)
+    basic, at_hi = col == 1, col == 2
+    at_lo = col == 0
+    if any(sF.values()):
+        raise NotCertified("a basic row slack is nonzero")
+    # exact KKT
     Ax = [Fraction(0)] * m
     for j in range(n):
         if xF[j]:
@@ -211,6 +309,7 @@ def exact_optimum(t, cparams_row, rparams_row, basis=None) -> ExactOptimum:
         if at_hi[j] and rF[j] > 0:
             raise NotCertified(f"column {j} at its bound with a positive reduced cost")
     objF = sum((cF[j] * xF[j] for j in range(n) if xF[j]), Fraction(0)) + _objective_constant(t, cp, rp)
+    bidx = np.flatnonzero(basic)
     inside = [min(xF[j], uF[j] - xF[j]) if fin[j] else xF[j] for j in bidx]
     sc = max(1e-300, float(np.abs(c).max(initial=0.0)))
     x = np.array([float(v) for v in xF])
@@ -220,7 +319,7 @@ def exact_optimum(t, cparams_row, rparams_row, basis=None) -> ExactOptimum:
                         x_margin=float(min(inside, default=math.inf)) / max(1.0, float(np.abs(x).max(initial=0.0))),
                         r_margin=float(min((abs(rF[j]) for j in range(n) if not basic[j]), default=math.inf)) / sc,
                         r=np.array([float(v) for v in rF]), fixed=np.array([v != 0 for v in rF]),
-                        inside=np.array([xF[j] > 0 and (not fin[j] or xF[j] < uF[j]) for j in range(n)]))
+                        inside=np.array([xF[j] > 0 and (not fin[j] or xF[j] < uF[j]) for j in range(n)]), pivots=pivots)
 
 
 def kkt_residuals(t, cparams_row, rparams_row, x, y, lp_zero=False):

@@ -4,7 +4,11 @@ The LPs the project solves are primal and dual degenerate: a quarter of the hour
 idle, capacity factors are 0.  Their x and y are then not unique, and the planted generators (planted_stage.py) cannot stand in
 for them.  Each set here is built deterministically from the committed price / capacity-factor pool (dispatches_b200/data) and
 the scenario batches of dispatches_b200/scenarios.py, certified LP by LP with exact_lp.exact_optimum (HiGHS' final basis,
-verified in exact arithmetic) and cached per process.
+verified in exact arithmetic, or its exact repair) and cached per process.  The sets cover the wind + battery dispatch (C2, C5,
+real windows of 2 to 256 hours, the edges), nuclear, fossil, wind + battery + PEM, the double-loop operation LPs, battery design,
+and PV + battery + hydrogen at fixed sizes and in design (one PV series baked into A, or one per LP as matrix coefficients).  Not
+covered: the free-wind design, which HiGHS reports unbounded at 1e-10 tolerances, and the full-year LP, whose exact certification
+takes over a minute.
 
 ``check_exact`` measures a kernel's answer on such a set against what every optimum of the LP shares: the objective, the KKT
 conditions, x / y element-wise where they are unique, and on every LP the columns every optimal x has at a bound (``fixed``)
@@ -14,7 +18,9 @@ from __future__ import annotations
 
 import dataclasses
 import functools
+import json
 import multiprocessing as mp
+from pathlib import Path
 
 import numpy as np
 
@@ -51,6 +57,7 @@ class ExactSet:
     csc: np.ndarray            # [N] |c|_inf
     x_margin: np.ndarray       # [N] ExactOptimum.x_margin
     r_margin: np.ndarray       # [N] ExactOptimum.r_margin
+    pivots: np.ndarray         # [N] ExactOptimum.pivots: exact dual simplex pivots that repaired HiGHS' basis
 
     def __len__(self):
         return len(self.obj)
@@ -86,7 +93,7 @@ def certify(t, cparams, rparams, procs=1):
     st = lambda f: np.array([getattr(e, f) for e in es])
     return ExactSet(t, cparams, rparams, st("x"), st("y"), st("r"), st("obj"), st("lp_mag"), st("fixed"), st("inside"),
                     st("unique_x"), st("unique_y"), np.array([o[1] for o in out]), np.array([o[2] for o in out]), st("x_margin"),
-                    st("r_margin"))
+                    st("r_margin"), st("pivots"))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -234,6 +241,81 @@ def design(T=24, N=8):
     lmp, cf, W, _ = SC.c2(N, seed=8)
     lmp[::2] *= 40.0
     return certify(TP.wind_battery_design(T), lmp, TP.wind_battery_rparams(T, cf, W, 0.0))
+
+
+SOLAR_SIZES = ("no_battery", "battery", "battery_pem")
+
+
+def _solar_reference():
+    from oracle import lp_models as L
+    gold = json.load(open(Path(__file__).parent / "golden" / "solar_golden.json"))
+    return np.array(gold["lmp_24"]), L.solar_default_series()
+
+
+@functools.lru_cache(maxsize=None)
+def solar(sizes, N=8, T=24):
+    """PV + battery + hydrogen dispatch at fixed sizes (solar_battery_hydrogen, a band template), PV 200 MW: LP 0 is the reference's
+    case, the others scale its prices (lognormal), loads (0.7 .. 1.2) and capacity factors (0.5 .. 1.0) per hour.  ``sizes``:
+    no_battery (turbine and tank only), battery (50 MW / 200 MWh), battery_pem (and a 20 MW PEM).  The tank the reference sizes for
+    its reserve (100 MW / (0.39 x 33.391) kg) backs 8.6e-14 kW less than 100 MW in exact arithmetic, so without a battery the
+    night-time reserve rows make the reference's LP infeasible by that much: no_battery sizes the tank 1 % larger."""
+    lmp0, d = _solar_reference()
+    kw = {"no_battery": dict(tank_kg=1.01 * TP.solar_battery_hydrogen(T).meta["tank_kg"]),
+          "battery": dict(batt_mw=50.0, batt_mwh=200.0),
+          "battery_pem": dict(batt_mw=50.0, batt_mwh=200.0, pem_mw=20.0)}[sizes]
+    rng = np.random.default_rng([T, 9, SOLAR_SIZES.index(sizes)])
+    one = np.ones((1, T))
+    lmp = np.tile(lmp0, T // 24) * np.vstack([one, rng.lognormal(0.0, 0.3, (N - 1, T))])
+    load = np.tile(d["load_mw"], T // 24) * np.vstack([one, rng.uniform(0.7, 1.2, (N - 1, T))])
+    cfs = np.tile(d["pv_cfs"], T // 24) * np.vstack([one, rng.uniform(0.5, 1.0, (N - 1, T))])
+    return certify(TP.solar_battery_hydrogen(T, **kw), lmp, TP.solar_rparams(T, cfs, 200.0, load))
+
+
+@functools.lru_cache(maxsize=None)
+def solar_design(T=24, N=8, procs=1):
+    """the PV + battery + hydrogen design LP over the baked template solar_battery_hydrogen_design(T, pv_cfs) with the reference's
+    capacity factors (hour 12 of each day is sin(pi) = 1.2e-16, an entry of A that HiGHS drops): LP 0 is the reference's case, the
+    others scale its prices (lognormal) and loads (0.7 .. 1.2) per hour"""
+    lmp0, d = _solar_reference()
+    rng = np.random.default_rng([T, 10])
+    one = np.ones((1, T))
+    lmp = np.tile(lmp0, T // 24) * np.vstack([one, rng.lognormal(0.0, 0.3, (N - 1, T))])
+    load = 1e3 * np.tile(d["load_mw"], T // 24) * np.vstack([one, rng.uniform(0.7, 1.2, (N - 1, T))])
+    return certify(TP.solar_battery_hydrogen_design(T, np.tile(d["pv_cfs"], T // 24)), lmp, load, procs)
+
+
+SOLAR_PV = ("reference", "dyadic", "zero_hours", "all_zero", "cf_one", "reserve")
+
+
+def solar_pv_series(T, N):
+    """(lmp, load_mw, pv_cfs, reserve_mw) [N, T] of solar_design_pv, one row per SOLAR_PV case in that order, then perturbed series
+    with zero hours: the reference's case; a series on the 1/64 grid (that LP is the baked template's LP bit for bit); a quarter of
+    the hours exactly 0; an all-zero series; hours clipped at cf = 1; a perturbed reserve series"""
+    from test_design_pv_series import dyadic_cfs
+    lmp0, d = _solar_reference()
+    rng = np.random.default_rng([T, 11])
+    lmp = np.tile(lmp0, (N, T // 24))
+    load = np.tile(d["load_mw"], (N, T // 24))
+    cfs = np.tile(d["pv_cfs"], (N, T // 24))
+    reserve = np.tile(d["reserve_mw"], (N, T // 24))
+    lmp[2:] *= rng.lognormal(0.0, 0.3, (N - 2, T))
+    load[2:] *= rng.uniform(0.7, 1.2, (N - 2, T))
+    cfs[1] = dyadic_cfs(T, T)
+    for k in [2] + list(range(len(SOLAR_PV), N)):
+        cfs[k] *= rng.uniform(0.5, 1.0, T)
+        cfs[k, rng.choice(T, T // 4, replace=False)] = 0.0
+    cfs[3] = 0.0
+    cfs[4] = np.minimum(1.0, 1.5 * cfs[4])
+    reserve[5] *= rng.uniform(0.4, 1.0, T)
+    return lmp, load, cfs, reserve
+
+
+@functools.lru_cache(maxsize=None)
+def solar_design_pv(T=24, N=8, procs=1):
+    """the design LP with a PV and a reserve series per LP (solar_battery_hydrogen_design(T, None), per-problem matrix coefficients):
+    the series of solar_pv_series"""
+    lmp, load, cfs, reserve = solar_pv_series(T, N)
+    return certify(TP.solar_battery_hydrogen_design(T, None), lmp, TP.solar_design_rparams(T, load, cfs, reserve), procs)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -1,5 +1,6 @@
 """The dense kernel's algorithm on the CPU: the numpy mirror (oracle/ipm_dense_numpy.py) on the PV + battery + hydrogen design LP
-against HiGHS and the dense-Cholesky mirror, on planted LPs with w > 32 and a fully dense A against their exact optimum, and the CUDA
+against HiGHS and the dense-Cholesky mirror, on real, degenerate LPs against their exact optima (real_lps.check_exact: what the
+kernel must reach on the GPU), on planted LPs with w > 32 and a fully dense A against their exact optimum, and the CUDA
 tile routines of csrc/dsp_dense.cuh (blocked LDL', panel, tensor-core trailing update through its FMA fallback, substitutions) on
 the SIMT emulator against numpy -- including zero and negative pivots and sizes that are not a multiple of the tile."""
 import ctypes as C
@@ -13,6 +14,7 @@ import pytest
 
 from dispatches_b200 import templates as TP
 from oracle import highs as H, ipm_dense_numpy as ID, ipm_numpy as IN, lp_models as L
+import real_lps as R
 from planted_lp import planted, rel
 
 HERE = Path(__file__).resolve().parent
@@ -29,6 +31,21 @@ def _design_batch(T, N, seed):
     lmp = np.vstack([lmp0[None], lmp0[None] * rng.lognormal(0, 0.3, (N - 1, T))])
     load = np.vstack([load0[None], load0[None] * rng.uniform(0.7, 1.2, (N - 1, T))])
     return lmp, load, cfs
+
+
+@pytest.mark.parametrize("name", ["solar_design24", "solar_design_pv24", "wb17"])
+def test_mirror_on_exact_optima(name):
+    """the design LP baked and with a PV series per LP (each LP's own matrix), and wind + battery windows with m = 68 (one row past
+    a 64-row tile) through check_exact with the GPU suite's bars"""
+    s = {"solar_design24": lambda: R.solar_design(24), "solar_design_pv24": lambda: R.solar_design_pv(24),
+         "wb17": lambda: R.windows(17)}[name]()
+    obj, status, x, y = [], [], [], []
+    for k in range(len(s)):
+        c, b, u, kk = s.t.instantiate(s.cparams[k], s.rparams[k])
+        r = ID.solve_batch(s.t.matrix(s.rparams[k]), b[None], c[None], u[None], rho=s.t.meta.get("reg_primal", 1e-8))
+        obj.append(r["obj"][0] + kk); status.append(r["status"][0]); x.append(r["x"][0]); y.append(r["y"][0])
+    e = R.check_exact(s, np.array(obj), np.array(status), np.stack(x), np.stack(y), what=name)
+    print(name, R.fmt(e))
 
 
 @pytest.mark.parametrize("T,N", [(24, 16), (48, 4)])

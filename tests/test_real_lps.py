@@ -1,12 +1,15 @@
 """The exact reference on real, degenerate dispatch LPs (tests/real_lps.py), on the CPU: the basis certifier against today's
 answers on planted LPs, its certification rate on the real sets, a hand-built LP with a known primal and dual optimal face, a
-corrupted basis, and the CUDA sources of stage 2, the long-horizon kernel and the chain kernel on the lock-step SIMT emulator
+corrupted basis, the exact repair of an infeasible HiGHS basis (planted by hand, and on the PV + battery + hydrogen LPs), and the
+CUDA sources of stage 2, the long-horizon kernel and the chain kernel on the lock-step SIMT emulator
 (tests/emu) through check_exact."""
 import numpy as np
 import pytest
 
+import exact_lp as X
 import real_lps as R
 from dispatches_b200 import lp_template as LT
+from dispatches_b200 import templates as TP
 from exact_lp import NotCertified, exact_optimum, highs_basis, kkt_residuals
 from planted_stage import XY_REL, planted_chain, planted_wb
 from test_planted_stage import _harness, needs_gxx
@@ -63,6 +66,127 @@ def test_real_sets_certify(name):
         assert not s.unique_y.all()
     e = R.check_exact(s, s.obj, np.zeros(len(s), np.int32), s.x, s.y, what=name)
     assert max(e["primal"], e["bound"]) < 1e-14
+    assert (s.pivots == 0).all()
+
+
+EXISTING = {"c2": lambda: R.c2(64), "c5": R.c5, "edges": R.edges, "windows33": lambda: R.windows(33), "nuclear": lambda: R.nuclear(48),
+            "nuclear_report": lambda: R.nuclear_report(48), "fossil": lambda: R.fossil(168, 4), "design": R.design,
+            "pem": lambda: R.wind_battery_pem(24, True), **{o: (lambda o=o: R.operation(o)) for o in R.OPERATIONS}}
+
+
+@pytest.mark.parametrize("name", sorted(EXISTING))
+def test_existing_sets_need_no_repair(name):
+    """HiGHS' basis verifies as it is on the sets that certified before the repair existed: no pivot, and on a sample of each set
+    the same ExactOptimum, bit for bit, as the verification of that basis without any repair (an explicit ``basis=``)"""
+    s = EXISTING[name]()
+    assert (s.pivots == 0).all()
+    for k in np.linspace(0, len(s) - 1, 3).astype(int):
+        e = exact_optimum(s.t, s.cparams[k], s.rparams[k])
+        c, b, u, _ = s.t.instantiate(s.cparams[k], s.rparams[k])
+        A = s.t.matrix(s.rparams[k]).tocsc(copy=True)
+        A.sort_indices()
+        f = exact_optimum(s.t, s.cparams[k], s.rparams[k], basis=highs_basis(c, A, b, u))
+        assert e.pivots == f.pivots == 0
+        for a, g in ((e.x, s.x[k]), (e.y, s.y[k]), (e.r, s.r[k]), (e.x, f.x), (e.y, f.y), (e.r, f.r), (e.basic, f.basic),
+                     (e.fixed, f.fixed), (e.inside, f.inside)):
+            assert np.array_equal(a, g)
+        assert (e.obj, e.lp_mag, e.unique_x, e.unique_y, e.x_margin, e.r_margin) == (f.obj, f.lp_mag, f.unique_x, f.unique_y,
+                                                                                      f.x_margin, f.r_margin)
+
+
+SOLAR = {**{f"solar_{z}": (lambda z=z: R.solar(z)) for z in R.SOLAR_SIZES}, "solar_design24": lambda: R.solar_design(24),
+         "solar_design48": lambda: R.solar_design(48), "solar_design_pv24": lambda: R.solar_design_pv(24),
+         "solar_design_pv48": lambda: R.solar_design_pv(48)}
+
+
+@pytest.mark.parametrize("name", sorted(SOLAR))
+def test_solar_sets_certify(name):
+    """the PV + battery + hydrogen LPs certify only through the repair: HiGHS drops the 1.2e-16 entry of sin(pi) or leaves row slacks
+    and basic columns 1e-14 .. 1e-11 outside their bounds in exact arithmetic.  They are degenerate in x and y."""
+    s = SOLAR[name]()
+    assert len(s) == 8 and s.pivots.max() > 0 and s.pivots.max() <= X.MAX_PIVOTS
+    assert not s.unique_x.any() and not s.unique_y.any()
+    e = R.check_exact(s, s.obj, np.zeros(len(s), np.int32), s.x, s.y, what=name)
+    assert max(e["primal"], e["bound"]) < 1e-13              # x* rounded to binary64: holdups of 1e6 mol next to flows of 1e-2
+    if name.startswith("solar_design") and "_pv" not in name:
+        assert 0.0 < np.abs(s.t.A.data).min() < 1e-15                # the sin(pi) hour, as the kernels receive it
+
+
+@pytest.mark.parametrize("T", [24, 48])
+def test_solar_pv_series_have_their_cases(T):
+    """the per-LP series hold exact zero hours, an all-zero series, cf = 1 hours and a perturbed reserve; the dyadic LP is the baked
+    template's LP, and its exact optimum is the baked one's bit for bit"""
+    lmp, load, cfs, reserve = R.solar_pv_series(T, 8)
+    case = {c: i for i, c in enumerate(R.SOLAR_PV)}
+    assert (cfs[case["zero_hours"]] == 0).sum() >= T // 4 and (cfs[case["all_zero"]] == 0).all() and (cfs[case["cf_one"]] == 1).any()
+    assert (reserve[case["reserve"]] != 100.0).all() and (reserve[np.arange(8) != case["reserve"]] == 100.0).all()
+    assert np.array_equal(cfs[case["reference"]], np.tile(R._solar_reference()[1]["pv_cfs"], T // 24))
+    s = R.solar_design_pv(T)
+    k = case["dyadic"]
+    tb = TP.solar_battery_hydrogen_design(T, cfs[k])
+    e = exact_optimum(tb, lmp[k], load[k] * 1e3)
+    assert np.array_equal(e.x, s.x[k]) and np.array_equal(e.y, s.y[k]) and e.obj == s.obj[k]
+
+
+def test_reference_tank_without_battery_is_infeasible_in_exact_arithmetic():
+    """the reference sizes the tank for exactly its 100 MW reserve: in binary64 that tank backs 8.6e-14 kW less, and with no battery
+    the night-time reserve rows cannot be met.  The repair proves it (its ratio test finds no entering column), which is why
+    real_lps.solar sizes that tank 1 % larger."""
+    lmp0, d = R._solar_reference()
+    with pytest.raises(NotCertified, match="infeasible in exact arithmetic"):
+        exact_optimum(TP.solar_battery_hydrogen(24), lmp0, TP.solar_rparams(24, d["pv_cfs"], 200.0, d["load_mw"])[0])
+
+
+def _cover_lp(b, surplus):
+    """min x1 + 2 x2  s.t.  x1 + x2 - s = b (surplus: a column s >= 0) or x1 + x2 = b, x >= 0.  Optimum x1 = b, y = 1."""
+    B = LT.TemplateBuilder("cover", Pc=1, Pr=0)
+    x1, x2 = B.var("x1"), B.var("x2")
+    B.cost(x1, 1.0); B.cost(x2, 2.0)
+    row = {x1: 1.0, x2: 1.0}
+    if surplus:
+        row[B.var("s")] = -1.0
+    B.eq("r", row, b)
+    return B.build()
+
+
+@pytest.mark.parametrize("surplus", [True, False], ids=["basic_column", "basic_row_slack"])
+def test_repair_of_a_planted_basis(monkeypatch, surplus):
+    """HiGHS' basis replaced by a dual feasible one that is 1e-9 primal infeasible -- the surplus column basic at -b, or the row's
+    slack basic at b -- is repaired in one pivot to the exact optimum x1 = b, y = 1.  Given explicitly, the same basis raises; 1e-7
+    off, it is too far to repair."""
+    t = _cover_lp(1e-9, surplus)
+    col = np.zeros(t.n, np.int8)
+    if surplus:
+        col[t.col_names.index("s")] = 1
+    planted = (col, np.array([not surplus]))
+    monkeypatch.setattr(X, "highs_basis", lambda *a: planted)
+    e = exact_optimum(t, np.zeros(1), None)
+    assert e.pivots == 1 and e.x[t.col_names.index("x1")] == 1e-9 and e.x[t.col_names.index("x2")] == 0.0
+    assert e.y[0] == 1.0 and e.obj == 1e-9 and e.basic[t.col_names.index("x1")]
+    with pytest.raises(NotCertified):
+        exact_optimum(t, np.zeros(1), None, basis=planted)
+    with pytest.raises(NotCertified, match="too far to repair"):
+        exact_optimum(_cover_lp(1e-7, surplus), np.zeros(1), None)
+
+
+def test_repair_refuses_a_dual_infeasible_basis(monkeypatch):
+    """min x1 + 2 x2 - x3  s.t.  x1 + x2 = 1e-9,  x3 + x4 = 1: the basis {row slack 0, x4} is 1e-9 primal infeasible and dual
+    infeasible (x3 at 0 with r = -1) -- the repair does not start"""
+    B = LT.TemplateBuilder("two_rows", Pc=1, Pr=0)
+    v = [B.var(f"x{j}") for j in range(1, 5)]
+    B.cost(v[0], 1.0); B.cost(v[1], 2.0); B.cost(v[2], -1.0)
+    B.eq("r0", {v[0]: 1.0, v[1]: 1.0}, 1e-9)
+    B.eq("r1", {v[2]: 1.0, v[3]: 1.0}, 1.0)
+    t = B.build()
+    col = np.zeros(t.n, np.int8)
+    col[t.col_names.index("x4")] = 1
+    rb = np.array([n == "r0" for n in t.row_names])
+    monkeypatch.setattr(X, "highs_basis", lambda *a: (col, rb))
+    with pytest.raises(NotCertified, match="primal and dual infeasible"):
+        exact_optimum(t, np.zeros(1), None)
+    monkeypatch.undo()
+    e = exact_optimum(t, np.zeros(1), None)
+    assert e.obj == -1.0 + 1e-9 and e.pivots == 0
 
 
 def test_edge_set_has_its_edges():

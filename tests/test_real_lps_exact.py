@@ -99,7 +99,7 @@ def test_chain(Lg, report):
 
 BAND = {"wb24": lambda: R.c2(64), "wb96": lambda: R.windows(96), "edges": R.edges, "pem": lambda: R.wind_battery_pem(24, True),
         "pem_nobatt": lambda: R.wind_battery_pem(24, False), "fossil": lambda: R.fossil(168), "design": R.design,
-        **{o: (lambda o=o: R.operation(o)) for o in R.OPERATIONS}}
+        **{o: (lambda o=o: R.operation(o)) for o in R.OPERATIONS}, **{f"solar_{z}": (lambda z=z: R.solar(z)) for z in R.SOLAR_SIZES}}
 
 
 @pytest.mark.parametrize("name", sorted(BAND))
