@@ -90,11 +90,12 @@ DNS void tile_panel8(const double *S, double *B, int row0, int lane) {
     }
 }
 
-// 8-row strip of a trailing update: C[row0 .. row0+8)[:] -= A[row0 .. row0+8)[:] * B'  (A, B staged, stride LDS; C in the workspace,
-// stride TS): 8 column blocks x 16 k-steps of mma m8n8k4, the strip of C in registers
+// 8-row strip of a trailing update: C[row0 .. row0+8)[:] -= A[row0 .. row0+8)[:] * B'  (A, B staged, stride LDS; C with row stride
+// LDC: a workspace tile, or a staged one): 8 column blocks x 16 k-steps of mma m8n8k4, the strip of C in registers
+template <int LDC = TS>
 DNS void tile_update8(double *C, const double *A, const double *B, int row0, int lane) {
     const int g = lane >> 2, t = lane & 3;
-    double *cr = C + (row0 + g) * TS + 2 * t;
+    double *cr = C + (row0 + g) * LDC + 2 * t;
     double acc[16];
 #pragma unroll
     for (int nb = 0; nb < 8; ++nb) { acc[2 * nb] = cr[nb * 8]; acc[2 * nb + 1] = cr[nb * 8 + 1]; }
@@ -204,6 +205,94 @@ DNS void solve(const double *G, int nt, const double *dinv, double *v, int warp,
         DENSE_SYNC();
         for (int J = warp; J < K; J += nwarps)
             tile_gemvt_sub(G + (long long)tile_index(K, J) * TILE, v + K * TS, dinv + J * TS, v + J * TS, lane);
+        DENSE_SYNC();
+    }
+}
+
+// ---- one LP per thread-block cluster (dsp_ipm_dense_cluster_kernel, m <= 4096)
+// The C ranks (CTAs) of a cluster share the lower tiles G, dinv and the substitution vector v of their LP.  Tile row I belongs to
+// rank I mod C.  The factorisation and the substitutions run in phases separated by cluster barriers.  Invariant: inside a phase a
+// rank writes only tiles and entries of v of its own rows (and the owner of a diagonal block its dinv block), and reads only what
+// earlier phases finished.  So the ranks may as well run one after another between the barriers (tests/emu does), and the result does
+// not depend on C.  Every tile also sees the operations of `factor` / `solve` in the same order, so the factor and the solution are
+// bitwise those of the single-CTA routines.
+constexpr int kGroup = 2;          // target tiles a rank accumulates together
+
+// the first tile row I >= J that rank `rank` of C owns (nt or more: none)
+DNS int first_own(int J, int rank, int C) { return J + ((rank - J % C) % C + C) % C; }
+
+// factorisation phase 1 of block column J on rank `rank`: each of its target tiles (I, J), I >= J, becomes
+// A(I,J) - sum_{K<J} W(I,K) D_K^-1 W(J,K)', accumulated over K in ascending order in a staged buffer and written back once (left-looking,
+// Crout order); the owner of (J, J) then factors it into L_JJ and dinv_J.  W(J,K) is staged once per group of kGroup target tiles.
+// SB: one staged-tile buffer; SC, SA: kGroup buffers each, TS * LDS doubles apart
+DNS void cluster_column(double *G, int nt, int J, int rank, int C, double *SB, double *SC, double *SA, double *dinv, int warp, int nwarps,
+                        int lane) {
+    const int tid = warp * 32 + lane, nthr = nwarps * 32;
+    for (int I0 = first_own(J, rank, C); I0 < nt; I0 += C * kGroup) {
+        const int left = (nt - 1 - I0) / C + 1, ng = left < kGroup ? left : kGroup;
+        DENSE_SYNC();
+        for (int g = 0; g < ng; ++g) stage_in(SC + g * TS * LDS, G + (long long)tile_index(I0 + g * C, J) * TILE, nullptr, tid, nthr);
+        for (int K = 0; K < J; ++K) {
+            DENSE_SYNC();
+            stage_in(SB, G + (long long)tile_index(J, K) * TILE, nullptr, tid, nthr);
+            for (int g = 0; g < ng; ++g)
+                stage_in(SA + g * TS * LDS, G + (long long)tile_index(I0 + g * C, K) * TILE, dinv + K * TS, tid, nthr);
+            DENSE_SYNC();
+            for (int g = 0; g < ng; ++g)
+                for (int s = warp; s < TS / 8; s += nwarps) tile_update8<LDS>(SC + g * TS * LDS, SA + g * TS * LDS, SB, s * 8, lane);
+        }
+        DENSE_SYNC();
+        if (I0 == J && warp == 0) tile_factor(SC, dinv + J * TS, lane);
+        DENSE_SYNC();
+        for (int g = 0; g < ng; ++g) stage_out(G + (long long)tile_index(I0 + g * C, J) * TILE, SC + g * TS * LDS, tid, nthr);
+    }
+}
+
+// factorisation phase 2 of block column J on rank `rank`: its tiles below the diagonal become W = A L_JJ^-T (L_JJ from phase 1)
+DNS void cluster_panel(double *G, int nt, int J, int rank, int C, double *SA, double *SB, int warp, int nwarps, int lane) {
+    const int tid = warp * 32 + lane, nthr = nwarps * 32;
+    const int I0 = first_own(J + 1, rank, C);
+    if (I0 >= nt) return;
+    DENSE_SYNC();
+    stage_in(SA, G + (long long)tile_index(J, J) * TILE, nullptr, tid, nthr);
+    for (int I = I0; I < nt; I += C) {
+        double *GIJ = G + (long long)tile_index(I, J) * TILE;
+        DENSE_SYNC();
+        stage_in(SB, GIJ, nullptr, tid, nthr);
+        DENSE_SYNC();
+        for (int s = warp; s < TS / 8; s += nwarps) tile_panel8(SA, SB, s * 8, lane);
+        DENSE_SYNC();
+        stage_out(GIJ, SB, tid, nthr);
+    }
+}
+
+// forward substitution phase K (0 <= K < nt) on rank `rank`: its rows I >= K take the update of block K-1, then the owner of row K
+// finishes it (L t = v, v <- dinv t, as in `solve`)
+DNS void cluster_fwd(const double *G, int nt, int K, int rank, int C, const double *dinv, double *v, int warp, int nwarps, int lane) {
+    if (K > 0) {
+        int c = 0;
+        for (int I = first_own(K, rank, C); I < nt; I += C, ++c)
+            if (c % nwarps == warp) tile_gemv_sub(G + (long long)tile_index(I, K - 1) * TILE, v + (K - 1) * TS, v + I * TS, lane);
+        DENSE_SYNC();
+    }
+    if (K % C == rank) {
+        if (warp == 0) tile_fwd(G + (long long)tile_index(K, K) * TILE, dinv + K * TS, v + K * TS, lane);
+        DENSE_SYNC();
+    }
+}
+
+// backward substitution phase K (nt > K >= 0) on rank `rank`: its rows J <= K take the update of block K+1, then the owner of row K
+// finishes it (L' v = v)
+DNS void cluster_bwd(const double *G, int nt, int K, int rank, int C, const double *dinv, double *v, int warp, int nwarps, int lane) {
+    if (K + 1 < nt) {
+        int c = 0;
+        for (int J = rank; J <= K; J += C, ++c)
+            if (c % nwarps == warp)
+                tile_gemvt_sub(G + (long long)tile_index(K + 1, J) * TILE, v + (K + 1) * TS, dinv + J * TS, v + J * TS, lane);
+        DENSE_SYNC();
+    }
+    if (K % C == rank) {
+        if (warp == 0) tile_bwd(G + (long long)tile_index(K, K) * TILE, v + K * TS, lane);
         DENSE_SYNC();
     }
 }

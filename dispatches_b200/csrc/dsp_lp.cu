@@ -17,6 +17,8 @@
 //
 // Kernel `dsp_ipm_dense_kernel` (any bandwidth, m <= 1024; dsp_lp_template_create_dense or DSP_KERNEL_DENSE): the same iteration,
 // one CTA per LP, M = A D A' dense in a workspace, blocked LDL' with FP64 tensor-core trailing updates (dsp_dense.cuh).
+// Kernel `dsp_ipm_dense_cluster_kernel` (m <= 4096; dsp_lp_template_create_dense_cluster or DSP_KERNEL_DENSE_CLUSTER): the same, one
+// thread-block cluster per LP, the factorisation and substitutions split over its CTAs by tile row.
 #include "dsp_lp.h"
 
 #include <cuda_runtime.h>
@@ -538,6 +540,7 @@ struct DParams {
     const double *am_coef;
     const int *at_from;                // CSC position -> CSR position
     const int *asm_qa, *asm_qb;        // assembly product q = A_val[asm_qa[q]] * A_val[asm_qb[q]]
+    long long rank_doubles;            // cluster kernel: doubles of a rank's own region (cta_doubles: of a cluster's region)
 };
 
 
@@ -551,9 +554,18 @@ struct DWork {
     double *s, *wv, *u, *ru, *cors, *rs;
     double *y, *b, *rp;
     double *dy, *dinv;                 // mp
-    double *G;                         // lower tiles of M
+    double *G;                         // lower tiles of M (cluster kernel: the rank's own region, mat_off is relative to it)
     double *SA, *SB, *red;
+    // cluster kernel: the cluster's lower tiles and substitution vector, kGroup target-tile buffers, this CTA's rank of csize
+    double *Gc, *vs, *SC;
+    int rank, csize;
 };
+
+// cluster barrier with release / acquire semantics: the global and shared memory writes of every CTA of the cluster before it are
+// visible to every CTA after it
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
 
 __device__ __forceinline__ double cta_max(double v, double *red) {
     v = warp_max(v);
@@ -585,7 +597,27 @@ __device__ __forceinline__ const double *dense_At(const DWork &W, const DParams 
 template <bool PerLP>
 __device__ __forceinline__ const double *dense_asm(const DWork &W, const DParams &P) { return PerLP ? W.G + P.mat_off + 2 * P.nnz : P.asm_val; }
 
-template <bool CORR, bool PerLP>
+// M v = r over the cluster (cluster kernel): every rank holds the same r in W.dy; the owner of a tile row publishes it in the cluster's
+// vector, the phases of dsp_dense.cuh run between cluster barriers, and every rank takes the whole solution back
+__device__ void dense_cluster_solve(const DWork &W, const DParams &P, int tid) {
+    const int nt = P.nt, warp = tid >> 5, lane = tid & 31;
+    cluster_sync();                                           // every rank has read the cluster's vector of the last solve
+    for (int I = W.rank; I < nt; I += W.csize)
+        for (int k = tid; k < dense::TS; k += kDenseThreads) W.vs[I * dense::TS + k] = W.dy[I * dense::TS + k];
+    __syncthreads();
+    for (int K = 0; K < nt; ++K) {
+        dense::cluster_fwd(W.Gc, nt, K, W.rank, W.csize, W.dinv, W.vs, warp, kDenseWarps, lane);
+        cluster_sync();
+    }
+    for (int K = nt - 1; K >= 0; --K) {
+        dense::cluster_bwd(W.Gc, nt, K, W.rank, W.csize, W.dinv, W.vs, warp, kDenseWarps, lane);
+        cluster_sync();
+    }
+    for (int i = tid; i < nt * dense::TS; i += kDenseThreads) W.dy[i] = W.vs[i];
+    __syncthreads();
+}
+
+template <bool CORR, bool PerLP, bool Clu = false>
 __device__ void dense_newton(const DWork &W, const DParams &P, double smu, int tid) {
     const int n = P.n, nb = P.nb, m = P.m, mp = P.nt * dense::TS;
     for (int j = tid; j < nb; j += kDenseThreads) {
@@ -610,7 +642,8 @@ __device__ void dense_newton(const DWork &W, const DParams &P, double smu, int t
         W.dy[i] = acc;
     }
     __syncthreads();
-    dense::solve(W.G, P.nt, W.dinv, W.dy, tid >> 5, kDenseWarps, tid & 31);
+    if constexpr (Clu) dense_cluster_solve(W, P, tid);
+    else dense::solve(W.G, P.nt, W.dinv, W.dy, tid >> 5, kDenseWarps, tid & 31);
     for (int j = tid; j < n; j += kDenseThreads) {
         double acc = 0.0;
         for (int q = P.At_ptr[j]; q < P.At_ptr[j + 1]; ++q) acc += dense_At<PerLP>(W, P)[q] * W.dy[P.At_idx[q]];
@@ -660,12 +693,15 @@ __device__ void dense_load_matrix(const DWork &W, const DParams &P, long long p,
     __syncthreads();
 }
 
-// one attempt on LP p: the band kernel's solve_one (same scaling, start point, proximal term, stopping rule, results rules)
-template <bool PerLP>
+// one attempt on LP p: the band kernel's solve_one (same scaling, start point, proximal term, stopping rule, results rules).  Clu: the
+// cluster kernel -- every rank runs the element-wise and CSR passes on its own copy of the vectors (the same code, so the same
+// values), the assembly, factorisation and substitutions are split over the cluster, rank 0 writes the results
+template <bool PerLP, bool Clu = false>
 __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, double step_frac, double reg, int it0, int *status_out,
                                 int *iters_out) {
     const int n = P.n, nb = P.nb, m = P.m, nt = P.nt, mp = nt * dense::TS;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const bool lead = !Clu || W.rank == 0;
     const double *cp = P.cparams + p * (long long)P.Pc;
     const double *rp_ = P.rparams + p * P.rstride;
     double cmax = 0.0, bmax = 0.0, kconst = 0.0;
@@ -720,8 +756,10 @@ __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, d
     const double nrm_b = 1.0 + bsmax, nrm_c = 1.0 + (cmax > 0.0 ? 1.0 : 0.0);
     const double ntot = (double)(n + nb);
     if (__syncthreads_or(bad_u)) {
-        if (tid == 0) { P.obj[p] = __longlong_as_double(0x7ff8000000000000LL); P.status[p] = DSP_INFEASIBLE; P.iters[p] = it0; }
-        dsp_nan_rows(P.x_out, n, P.y_out, m, p, tid, kDenseThreads);
+        if (lead) {
+            if (tid == 0) { P.obj[p] = __longlong_as_double(0x7ff8000000000000LL); P.status[p] = DSP_INFEASIBLE; P.iters[p] = it0; }
+            dsp_nan_rows(P.x_out, n, P.y_out, m, p, tid, kDenseThreads);
+        }
         *status_out = DSP_OPTIMAL;          // no second attempt
         *iters_out = it0;
         return;
@@ -782,18 +820,38 @@ __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, d
         }
         if (it == P.max_iter) break;
         // ---- assemble the lower tiles of M = A D A' (padding rows: decoupled unit rows) and factor them
-        for (long long e = tid; e < ntd; e += kDenseThreads) W.G[e] = 0.0;
-        __syncthreads();
-        for (int e = tid; e < P.nent; e += kDenseThreads) {
-            double acc = 0.0;
-            for (int q = P.asm_ptr[e]; q < P.asm_ptr[e + 1]; ++q) acc += dense_asm<PerLP>(W, P)[q] * W.d[P.asm_col[q]];
-            W.G[P.asm_pos[e]] = acc;
+        if constexpr (Clu) {
+            const int ct = W.rank * kDenseThreads + tid, cn = W.csize * kDenseThreads;
+            for (long long e = ct; e < ntd; e += cn) W.Gc[e] = 0.0;
+            cluster_sync();
+            for (int e = ct; e < P.nent; e += cn) {
+                double acc = 0.0;
+                for (int q = P.asm_ptr[e]; q < P.asm_ptr[e + 1]; ++q) acc += dense_asm<PerLP>(W, P)[q] * W.d[P.asm_col[q]];
+                W.Gc[P.asm_pos[e]] = acc;
+            }
+            for (int i = m + ct; i < mp; i += cn)
+                W.Gc[(long long)dense::tile_index(i / dense::TS, i / dense::TS) * dense::TILE + (i % dense::TS) * (dense::TS + 1)] = 1.0;
+            cluster_sync();
+            for (int J = 0; J < nt; ++J) {
+                dense::cluster_column(W.Gc, nt, J, W.rank, W.csize, W.SB, W.SC, W.SA, W.dinv, warp, kDenseWarps, lane);
+                cluster_sync();
+                dense::cluster_panel(W.Gc, nt, J, W.rank, W.csize, W.SA, W.SB, warp, kDenseWarps, lane);
+                cluster_sync();
+            }
+        } else {
+            for (long long e = tid; e < ntd; e += kDenseThreads) W.G[e] = 0.0;
+            __syncthreads();
+            for (int e = tid; e < P.nent; e += kDenseThreads) {
+                double acc = 0.0;
+                for (int q = P.asm_ptr[e]; q < P.asm_ptr[e + 1]; ++q) acc += dense_asm<PerLP>(W, P)[q] * W.d[P.asm_col[q]];
+                W.G[P.asm_pos[e]] = acc;
+            }
+            for (int i = m + tid; i < mp; i += kDenseThreads)
+                W.G[(long long)dense::tile_index(i / dense::TS, i / dense::TS) * dense::TILE + (i % dense::TS) * (dense::TS + 1)] = 1.0;
+            dense::factor(W.G, nt, W.SA, W.SB, W.dinv, warp, kDenseWarps, lane);
         }
-        for (int i = m + tid; i < mp; i += kDenseThreads)
-            W.G[(long long)dense::tile_index(i / dense::TS, i / dense::TS) * dense::TILE + (i % dense::TS) * (dense::TS + 1)] = 1.0;
-        dense::factor(W.G, nt, W.SA, W.SB, W.dinv, warp, kDenseWarps, lane);
         // ---- affine predictor
-        dense_newton<false, PerLP>(W, P, 0.0, tid);
+        dense_newton<false, PerLP, Clu>(W, P, 0.0, tid);
         double ip = 0.0, id = 0.0;
         dense_step_pass<false>(W, P, 0.0, tid, ip, id);
         ip = cta_max(ip, W.red); id = cta_max(id, W.red);
@@ -816,7 +874,7 @@ __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, d
         const double sg = mua / mu;
         const double smu = sg * sg * sg * mu;
         // ---- centring corrector
-        dense_newton<true, PerLP>(W, P, smu, tid);
+        dense_newton<true, PerLP, Clu>(W, P, smu, tid);
         ip = 0.0; id = 0.0;
         dense_step_pass<true>(W, P, smu, tid, ip, id);
         ip = cta_max(ip, W.red); id = cta_max(id, W.red);
@@ -839,17 +897,17 @@ __device__ void dense_solve_one(const DWork &W, const DParams &P, long long p, d
         __syncthreads();
     }
     // ---- results
-    if (tid == 0) {
+    if (tid == 0 && lead) {
         P.obj[p] = pobj * beta_b * beta_c + kconst;
         P.status[p] = status;
         P.iters[p] = it + it0;
     }
-    if (P.x_out) {
+    if (P.x_out && lead) {
         double *xo = P.x_out + p * (long long)n;
         if (P.xperm) { for (int j = tid; j < n; j += kDenseThreads) xo[P.xperm[j]] = W.x[j] * beta_b; }
         else { for (int j = tid; j < n; j += kDenseThreads) xo[j] = W.x[j] * beta_b; }
     }
-    if (P.y_out) {
+    if (P.y_out && lead) {
         double *yo = P.y_out + p * (long long)m;
         if (P.yperm) { for (int i = tid; i < m; i += kDenseThreads) yo[P.yperm[i]] = W.y[i] * beta_c; }
         else { for (int i = tid; i < m; i += kDenseThreads) yo[i] = W.y[i] * beta_c; }
@@ -885,6 +943,58 @@ __global__ void __launch_bounds__(kDenseThreads, 1) dsp_ipm_dense_kernel(const D
         // second attempt (shorter step, stronger proximal term) for the rare LP whose first attempt ends non-optimal
         dense_solve_one<PerLP>(W, P, (long long)t, P.step_frac, P.reg, 0, &st, &it0);
         if (st != DSP_OPTIMAL) dense_solve_one<PerLP>(W, P, (long long)t, 0.99, 10.0 * P.reg, it0, &st, &it0);
+    }
+}
+
+// =====================================================================================================
+// Dense cluster kernel `dsp_ipm_dense_cluster_kernel` (any bandwidth, m <= 4096; dsp_lp_template_create_dense_cluster or
+// DSP_KERNEL_DENSE_CLUSTER): one LP per thread-block cluster of C CTAs of kDenseWarps warps, persistent.  The iteration is
+// dense_solve_one's; the lower tiles of M, dinv and the substitution vector sit in a per-cluster workspace region, the left-looking
+// factorisation and the substitutions of dsp_dense.cuh are split over the ranks by tile row.  Every rank keeps its own copy of the
+// per-LP vectors (shared memory when they fit, else its own region) and, per-problem templates, of the LP's matrix values.
+// =====================================================================================================
+constexpr int kDenseClusterMaxM = 4096;
+// shared memory ahead of the vectors: reduction slots, one staged-tile buffer and kGroup target and operand buffers each
+constexpr size_t kDenseClusterSmemFixed = (size_t)(2 * kDenseWarps + (1 + 2 * dense::kGroup) * dense::TS * dense::LDS) * 8;
+// doubles of a cluster's region ahead of its ranks' regions: the tiles, dinv, the substitution vector, the ticket slot
+__host__ __device__ inline long long dense_cluster_head_doubles(int nt) { return dense::tiles_doubles(nt) + 2LL * nt * dense::TS + 8; }
+
+template <bool PerLP>
+__global__ void __launch_bounds__(kDenseThreads, 1) dsp_ipm_dense_cluster_kernel(const DParams P) {
+    extern __shared__ __align__(16) double dsm[];
+    DWork W;
+    unsigned rank, csize, cid;
+    asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
+    asm("mov.u32 %0, %%cluster_nctarank;" : "=r"(csize));
+    asm("mov.u32 %0, %%clusterid.x;" : "=r"(cid));
+    W.rank = (int)rank; W.csize = (int)csize;
+    W.red = dsm;
+    W.SB = dsm + 2 * kDenseWarps;
+    W.SC = W.SB + dense::TS * dense::LDS;
+    W.SA = W.SC + dense::kGroup * dense::TS * dense::LDS;
+    const int n = P.n, nb = P.nb, m = P.m, mp = P.nt * dense::TS;
+    double *cl = P.ws + (long long)cid * P.cta_doubles;
+    W.Gc = cl;
+    double *dinv = cl + dense::tiles_doubles(P.nt);
+    W.vs = dinv + mp;
+    unsigned long long *ticket = (unsigned long long *)(W.vs + mp);
+    W.G = cl + dense_cluster_head_doubles(P.nt) + (long long)rank * P.rank_doubles;
+    double *base = P.vec_in_smem ? W.SA + dense::kGroup * dense::TS * dense::LDS : W.G;
+    W.x = base; W.z = W.x + n; W.c = W.z + n; W.rd = W.c + n; W.d = W.rd + n; W.dx = W.d + n; W.cor = W.dx + n; W.rx = W.cor + n;
+    W.s = W.rx + n; W.wv = W.s + nb; W.u = W.wv + nb; W.ru = W.u + nb; W.cors = W.ru + nb; W.rs = W.cors + nb;
+    W.y = W.rs + nb; W.b = W.y + m; W.rp = W.b + m;
+    W.dy = W.rp + m;
+    W.dinv = dinv;
+    for (;;) {
+        if (rank == 0 && threadIdx.x == 0) __stcg(ticket, atomicAdd(P.ticket, 1ULL));
+        cluster_sync();
+        const unsigned long long t = __ldcg(ticket);
+        cluster_sync();                                       // every rank has read the slot before rank 0 writes the next ticket
+        if ((long long)t >= P.N) break;
+        int st, it0 = 0;
+        if (PerLP) dense_load_matrix(W, P, (long long)t, threadIdx.x);
+        dense_solve_one<PerLP, true>(W, P, (long long)t, P.step_frac, P.reg, 0, &st, &it0);
+        if (st != DSP_OPTIMAL) dense_solve_one<PerLP, true>(W, P, (long long)t, 0.99, 10.0 * P.reg, it0, &st, &it0);
     }
 }
 
@@ -1048,6 +1158,7 @@ struct dsp_template {
     cudaStream_t stream, stream2;
     std::atomic<int> busy;         // a host call is in flight on this handle (staging buffers, streams and ticket are per handle)
     bool dense_only;               // made by dsp_lp_template_create_dense: no band data, only the dense kernel runs
+    bool cluster_only;             // made by dsp_lp_template_create_dense_cluster: no band data, only the dense cluster kernel runs
     struct Dense {                 // the dense kernel's data (dense templates; band templates: built at the first DSP_KERNEL_DENSE call)
         bool ready;
         int nt, nent;
@@ -1135,6 +1246,7 @@ int template_init(dsp_template *T, const dsp_template_desc *D) {
     T->d_cp = T->d_rp = T->d_obj = T->d_x = T->d_y = nullptr; T->d_status = T->d_iters = nullptr;
     T->stream = nullptr; T->stream2 = nullptr; T->busy.store(0);
     T->dense_only = false;
+    T->cluster_only = false;
     memset(&T->dn, 0, sizeof(T->dn));
     CK(cudaGetDevice(&T->device));
     cudaDeviceProp prop;
@@ -1697,14 +1809,19 @@ static int launch_band(const dsp_template *T, KParams K, cudaStream_t st) {
     return launched(ctas, warps * 32, smem, warps);
 }
 
-// the dense kernel's data of a band template, built from its device copy of A at the first DSP_KERNEL_DENSE call
-static int ensure_dense(const dsp_template *T) {
+// the dense kernels' data of a band template, built from its device copy of A at the first DSP_KERNEL_DENSE or _DENSE_CLUSTER call
+static int ensure_dense(const dsp_template *T, bool cluster) {
     static std::mutex mu;
     std::lock_guard<std::mutex> lk(mu);
     const KParams &K = T->kp;
-    if (K.n_amap > 0) { g_err = "dsp_lp_solve_batch: DSP_KERNEL_DENSE does not take per-problem matrix coefficients"; return DSP_E_ARG; }
+    const char *kn = cluster ? "DSP_KERNEL_DENSE_CLUSTER" : "DSP_KERNEL_DENSE";
+    if (K.n_amap > 0) { g_err = std::string("dsp_lp_solve_batch: ") + kn + " does not take per-problem matrix coefficients"; return DSP_E_ARG; }
+    if (cluster && K.m > kDenseClusterMaxM) {
+        g_err = "dsp_lp_solve_batch: DSP_KERNEL_DENSE_CLUSTER needs m <= 4096 (m = " + std::to_string(K.m) + ")";
+        return DSP_E_ARG;
+    }
+    if (!cluster && K.m > kDenseMaxM) { g_err = "dsp_lp_solve_batch: DSP_KERNEL_DENSE needs m <= 1024 (m = " + std::to_string(K.m) + ")"; return DSP_E_ARG; }
     if (T->dn.ready) return 0;
-    if (K.m > kDenseMaxM) { g_err = "dsp_lp_solve_batch: DSP_KERNEL_DENSE needs m <= 1024 (m = " + std::to_string(K.m) + ")"; return DSP_E_ARG; }
     std::vector<unsigned char> hot(K.hot_bytes);
     CK(cudaMemcpy(hot.data(), K.hot_g, hot.size(), cudaMemcpyDeviceToHost));
     const double *val = (const double *)hot.data();
@@ -1715,7 +1832,7 @@ static int ensure_dense(const dsp_template *T) {
 
 // dense kernel: one persistent CTA per LP in flight, as many CTAs per SM as fit; the lower tiles of M of every CTA in the handle's
 // workspace, the per-LP vectors in shared memory when they fit next to the two staged-tile buffers (else behind the tiles)
-static int launch_dense(const dsp_template *T, const KParams &K, cudaStream_t st) {
+static DParams dense_params(const dsp_template *T, const KParams &K) {
     const dsp_template::Dense &D = T->dn;
     DParams Q;
     memset(&Q, 0, sizeof(Q));
@@ -1729,10 +1846,16 @@ static int launch_dense(const dsp_template *T, const KParams &K, cudaStream_t st
     Q.tol = K.tol; Q.feas_tol = K.feas_tol; Q.step_frac = K.step_frac; Q.reg = K.reg; Q.max_iter = K.max_iter;
     Q.obj = K.obj; Q.x_out = K.x_out; Q.y_out = K.y_out; Q.status = K.status; Q.iters = K.iters; Q.ticket = K.ticket;
     Q.xperm = K.xperm; Q.yperm = K.yperm;
-    const bool per_lp = D.n_amq > 0;
     Q.nnz = K.nnz; Q.n_amq = D.n_amq; Q.nterms = D.nterms;
     Q.am_q = D.am_q; Q.am_ptr = D.am_ptr; Q.am_param = D.am_param; Q.am_coef = D.am_coef;
     Q.at_from = D.at_from; Q.asm_qa = D.asm_qa; Q.asm_qb = D.asm_qb;
+    return Q;
+}
+
+static int launch_dense(const dsp_template *T, const KParams &K, cudaStream_t st) {
+    const dsp_template::Dense &D = T->dn;
+    DParams Q = dense_params(T, K);
+    const bool per_lp = D.n_amq > 0;
     const long long vec = dense_vec_doubles(K.m, K.n, K.nb, D.nt);
     Q.vec_in_smem = kDenseSmemFixed + (size_t)vec * 8 <= (size_t)T->smem_optin;
     const size_t smem = kDenseSmemFixed + (Q.vec_in_smem ? (size_t)vec * 8 : 0);
@@ -1749,6 +1872,43 @@ static int launch_dense(const dsp_template *T, const KParams &K, cudaStream_t st
     CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
     kern<<<(unsigned)ctas, kDenseThreads, smem, st>>>(Q);
     return launched(ctas, kDenseThreads, smem, 1);
+}
+
+// dense cluster kernel: one persistent cluster of C CTAs per LP in flight (C = 4 up to 32 tile rows, 8 above), as many clusters as
+// are co-resident; every cluster's region of the handle's workspace holds the LP's tiles, dinv and substitution vector, then each
+// rank's own per-LP vectors (when they do not fit in shared memory next to the staged-tile buffers) and matrix values (per-problem)
+static int launch_dense_cluster(const dsp_template *T, const KParams &K, cudaStream_t st) {
+    const dsp_template::Dense &D = T->dn;
+    DParams Q = dense_params(T, K);
+    const bool per_lp = D.n_amq > 0;
+    const int csize = D.nt <= 32 ? 4 : 8;
+    const long long vec = dense_vec_doubles(K.m, K.n, K.nb, D.nt);
+    Q.vec_in_smem = kDenseClusterSmemFixed + (size_t)vec * 8 <= (size_t)T->smem_optin;
+    const size_t smem = kDenseClusterSmemFixed + (Q.vec_in_smem ? (size_t)vec * 8 : 0);
+    Q.mat_off = Q.vec_in_smem ? 0 : vec;
+    Q.rank_doubles = Q.mat_off + (per_lp ? 2LL * K.nnz + D.nterms : 0);
+    Q.cta_doubles = dense_cluster_head_doubles(D.nt) + csize * Q.rank_doubles;     // per cluster
+    void (*kern)(DParams) = per_lp ? dsp_ipm_dense_cluster_kernel<true> : dsp_ipm_dense_cluster_kernel<false>;
+    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = csize; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3(csize); cfg.blockDim = dim3(kDenseThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    int ncl = 0;
+    CK(cudaOccupancyMaxActiveClusters(&ncl, (void *)kern, &cfg));
+    if (ncl < 1) { g_err = "dsp_lp_solve_batch: no cluster of " + std::to_string(csize) + " CTAs of the dense cluster kernel fits on the device"; return DSP_E_CUDA; }
+    long long clusters = std::min<long long>(K.N, ncl);
+    while (clusters > 1 && (size_t)clusters * Q.cta_doubles * 8 > T->ws_cap) clusters /= 2;
+    const int rc = grow_ws(T, (size_t)clusters * Q.cta_doubles * 8, st);
+    if (rc) return rc;
+    Q.ws = T->ws;
+    CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
+    cfg.gridDim = dim3((unsigned)(clusters * csize));
+    CK(cudaLaunchKernelEx(&cfg, kern, Q));
+    return launched(clusters * csize, kDenseThreads, smem, csize);
 }
 
 static int launch_batch(const dsp_template *T, int64_t N, const double *cparams, const double *rparams,
@@ -1769,12 +1929,22 @@ static int launch_batch(const dsp_template *T, int64_t N, const double *cparams,
     K.obj = obj; K.status = status; K.iters = iters; K.x_out = x; K.y_out = y;
     K.ticket = ticket;
     K.retry_only = 0;
+    if (T->cluster_only && o.kernel != DSP_KERNEL_AUTO && o.kernel != DSP_KERNEL_DENSE_CLUSTER) {
+        g_err = "dsp_lp_solve_batch: a template made by dsp_lp_template_create_dense_cluster runs only the dense cluster kernel (DSP_KERNEL_AUTO or DSP_KERNEL_DENSE_CLUSTER)";
+        return DSP_E_ARG;
+    }
+    if (T->cluster_only || o.kernel == DSP_KERNEL_DENSE_CLUSTER) {
+        if (T->dense_only) { g_err = "dsp_lp_solve_batch: a template made by dsp_lp_template_create_dense runs only the dense kernel (DSP_KERNEL_AUTO or DSP_KERNEL_DENSE)"; return DSP_E_ARG; }
+        const int rc = ensure_dense(T, true);
+        if (rc) return rc;
+        return launch_dense_cluster(T, K, st);
+    }
     if (T->dense_only && o.kernel != DSP_KERNEL_AUTO && o.kernel != DSP_KERNEL_DENSE) {
         g_err = "dsp_lp_solve_batch: a template made by dsp_lp_template_create_dense runs only the dense kernel (DSP_KERNEL_AUTO or DSP_KERNEL_DENSE)";
         return DSP_E_ARG;
     }
     if (T->dense_only || o.kernel == DSP_KERNEL_DENSE) {
-        const int rc = ensure_dense(T);
+        const int rc = ensure_dense(T, false);
         if (rc) return rc;
         return launch_dense(T, K, st);
     }
@@ -1900,7 +2070,7 @@ static int solve_batch_host_locked(dsp_template *T, int64_t N, const double *cpa
     cudaStream_t sts[2] = {T->stream, T->stream2};
     int64_t dstride = 0;
     // templates that run in global-workspace mode share ONE workspace: no concurrent chunk kernels for them
-    const bool dense = T->dense_only || (opts && opts->kernel == DSP_KERNEL_DENSE);            // the dense kernel always uses the workspace
+    const bool dense = T->dense_only || T->cluster_only || (opts && (opts->kernel == DSP_KERNEL_DENSE || opts->kernel == DSP_KERNEL_DENSE_CLUSTER));    // the dense kernels always use the workspace
     const bool ws_template = dense || band_geometry(T, K).ws || (T->has_stage && T->sp.T > kStage2MaxT);    // (the long stage kernel's workspace too)
     // Chunks pay when there is something to overlap: the staging memcpy of pageable input (always), or the H2D copy of a batch whose
     // kernel runs for many waves.  A page-locked batch of a few waves goes in ONE piece: the persistent stage kernels fill every SM
@@ -2153,14 +2323,19 @@ int dsp_lp_template_create_csr(const dsp_lp_desc *D, dsp_template **out) {
     return 0;
 }
 
-// dsp_lp_template_create_dense and its variant with per-problem matrix coefficients (count > 0); fn names the entry point in messages
+// dsp_lp_template_create_dense, its variant with per-problem matrix coefficients (count > 0) and (cluster) the dense cluster kernel's
+// dsp_lp_template_create_dense_cluster; fn names the entry point in messages
 static int create_dense(const char *fn, const dsp_lp_desc *D, int32_t count, const int32_t *row, const int32_t *col, const int32_t *param,
-                        const double *coef, dsp_template **out) {
+                        const double *coef, dsp_template **out, bool cluster = false) {
     const std::string f = fn;
     if (!out) { g_err = f + ": out is NULL"; return DSP_E_ARG; }
     if (!D || D->m <= 0 || D->n <= 0 || !D->A_ptr || !D->A_idx || !D->A_val || !D->u0) { g_err = f + ": bad descriptor"; return DSP_E_ARG; }
-    if (D->m > kDenseMaxM) {
+    if (!cluster && D->m > kDenseMaxM) {
         g_err = f + ": m = " + std::to_string(D->m) + " rows; the dense kernel takes m <= 1024";
+        return DSP_E_ARG;
+    }
+    if (cluster && D->m > kDenseClusterMaxM) {
+        g_err = f + ": m = " + std::to_string(D->m) + " rows; the dense cluster kernel takes m <= 4096";
         return DSP_E_ARG;
     }
     const int m = D->m, n = D->n, nnz = D->A_ptr[m];
@@ -2234,7 +2409,8 @@ static int create_dense(const char *fn, const dsp_lp_desc *D, int32_t count, con
     } guard{T};
     if (int rc = template_init(T, &d)) return rc;
     T->kp.w = w; T->kp.nnz = nnz;
-    T->dense_only = true;
+    T->dense_only = !cluster;
+    T->cluster_only = cluster;
     if (int rc = dense_build(T, A_ptr, A_idx, A_val, &terms)) return rc;
     T->col_perm = col_perm; T->row_perm = row_perm;
     int *dx = nullptr;
@@ -2255,10 +2431,15 @@ int dsp_lp_template_create_dense_with_matrix_params(const dsp_lp_desc *D, int32_
     return create_dense("dsp_lp_template_create_dense_with_matrix_params", D, count, row, col, param, coef, out);
 }
 
+int dsp_lp_template_create_dense_cluster(const dsp_lp_desc *D, int32_t count, const int32_t *row, const int32_t *col, const int32_t *param,
+                                         const double *coef, dsp_template **out) {
+    return create_dense("dsp_lp_template_create_dense_cluster", D, count, row, col, param, coef, out, true);
+}
+
 int dsp_lp_template_set_matrix_params(dsp_template *T, int32_t count, const int32_t *row, const int32_t *col, const int32_t *param,
                                       const double *coef) {
     if (!T || count < 0 || (count > 0 && (!row || !col || !param || !coef))) { g_err = "dsp_lp_template_set_matrix_params: bad arguments"; return DSP_E_ARG; }
-    if (T->dense_only) { g_err = "dsp_lp_template_set_matrix_params: per-problem matrix coefficients are not supported on a dense template"; return DSP_E_ARG; }
+    if (T->dense_only || T->cluster_only) { g_err = "dsp_lp_template_set_matrix_params: per-problem matrix coefficients are not supported on a dense template"; return DSP_E_ARG; }
     if (T->csr_ptr.empty()) { g_err = "dsp_lp_template_set_matrix_params: the template must come from dsp_lp_template_create_csr"; return DSP_E_ARG; }
     if (T->kp.w != 1 && T->kp.w != 2 && T->kp.w != 4 && T->kp.w != 8 && T->kp.w != 16 && T->kp.w != 32) { g_err = "bad band"; return DSP_E_ARG; }
     KParams &K = T->kp;

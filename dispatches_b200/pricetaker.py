@@ -22,7 +22,7 @@ import dataclasses
 import numpy as np
 
 from . import templates as TP
-from .solver import KERNEL_DENSE, BatchLPSolver, OPTIMAL, STATUS_NAMES
+from .solver import KERNEL_DENSE, KERNEL_DENSE_CLUSTER, BatchLPSolver, OPTIMAL, STATUS_NAMES
 
 _SOLVERS = {}
 
@@ -328,8 +328,12 @@ def pv_battery_hydrogen_design_optimize(n_time_points, input_params, verbose=Fal
     dict, one series).  With one PV and one reserve series (or N equal rows) the capacity factors are baked into the template; with a
     series per scenario they are per-problem matrix coefficients of the added-PV column (templates.solar_battery_hydrogen_design(T, None)),
     and the whole batch still runs in one launch.  Same ``input_params`` keys as ``re_h2_parameters``; ``pv_mw`` / ``turb_mw`` are the
-    existing PV and turbine sizes the design adds to.  The six size columns make A A' dense, so the LPs run on the dense kernel
-    (m <= 1024: T <= 48).  Returns (design_res, df) like the reference, with the optimal sizes per scenario."""
+    existing PV and turbine sizes the design adds to.  The six size columns make A A' dense, so the LPs run on the dense normal equations:
+    the dense kernel (one CTA per LP) while the LP has m = 15 T + 3 <= 1024 rows (T <= 68), the dense cluster kernel (one thread-block
+    cluster per LP) up to m <= 4096 (T <= 272); a longer horizon raises ValueError.  The reference annualises by weeks (revenue times
+    52 / n_weeks), so a week-long horizon sees the weekday / weekend pattern of the prices; a year of hourly prices is 52 such LPs in one
+    call, e.g. ``LMP = lmp_year[:8736].reshape(52, 168)`` with ``n_time_points = 168``.  Returns (design_res, df) like the reference, with
+    the optimal sizes per scenario."""
     T = int(n_time_points)
     for k in ("LMP", "pv_resource", "load", "reserve"):
         if k not in input_params:
@@ -355,25 +359,32 @@ def pv_battery_hydrogen_design_optimize(n_time_points, input_params, verbose=Fal
     kw = dict(pv_mw=float(input_params.get("pv_mw", 0.0)), turb_mw=float(input_params.get("turb_mw", 0.0)),
               max_sales=float(input_params.get("max_sales", 1000.0)), max_purchases=float(input_params.get("max_purchases", 1000.0)))
     lmp = np.ascontiguousarray(np.broadcast_to(lmp, (N, T)))
+    m = 15 * T + 3                                      # rows of the design LP (templates.solar_battery_hydrogen_design)
+    if m > 4096:
+        raise ValueError(f"pv_battery_hydrogen_design_optimize: n_time_points = {T} gives an LP of {m} rows; the dense kernels take "
+                         "m <= 4096 (n_time_points <= 272)")
+    kernel = KERNEL_DENSE if m <= 1024 else KERNEL_DENSE_CLUSTER
+    kname = "dense kernel" if kernel == KERNEL_DENSE else "dense cluster kernel"
     if np.all(cfs == cfs[:1]) and np.all(reserve == reserve[:1]):
         # one PV and one reserve series: baked into the template
         cf1, rs1 = np.ascontiguousarray(cfs[0]), np.ascontiguousarray(reserve[0])
         key = ("solar_battery_hydrogen_design", T, tuple(sorted(kw.items())), tuple(sorted(par.items())), cf1.tobytes(), rs1.tobytes())
         if key not in _SOLVERS:
-            _SOLVERS[key] = BatchLPSolver(TP.solar_battery_hydrogen_design(T, cf1, reserve_mw=rs1, par=par, **kw), kernel=KERNEL_DENSE)
+            _SOLVERS[key] = BatchLPSolver(TP.solar_battery_hydrogen_design(T, cf1, reserve_mw=rs1, par=par, **kw), kernel=kernel)
         rp = np.ascontiguousarray(np.broadcast_to(load * 1e3, (N, T)))
     else:
         # a series per scenario: cf_t multiplies the added-PV column -> per-problem matrix coefficients of the dense kernel
         key = ("solar_battery_hydrogen_design_pvbatched", T, tuple(sorted(kw.items())), tuple(sorted(par.items())))
         if key not in _SOLVERS:
-            _SOLVERS[key] = BatchLPSolver(TP.solar_battery_hydrogen_design(T, None, par=par, **kw), kernel=KERNEL_DENSE)
+            _SOLVERS[key] = BatchLPSolver(TP.solar_battery_hydrogen_design(T, None, par=par, **kw), kernel=kernel)
         rp = np.ascontiguousarray(TP.solar_design_rparams(T, np.broadcast_to(load, (N, T)), np.broadcast_to(cfs, (N, T)),
                                                           np.broadcast_to(reserve, (N, T))))
     sol = _SOLVERS[key]
     t = sol.t
+    assert t.m == m, (t.m, m)
     r = sol.solve_host(lmp, rp, want_x=True)
     if verbose:
-        print(f"b200ipm (dense kernel): {N} LPs, iterations mean {r.iters.mean():.1f} max {r.iters.max()}, "
+        print(f"b200ipm ({kname}): {N} LPs, iterations mean {r.iters.mean():.1f} max {r.iters.max()}, "
               f"non-optimal {(r.status != OPTIMAL).sum()}")
     xm = sol.to_model_space(r.x)
     names = {n: j for j, n in enumerate(t.col_names)}

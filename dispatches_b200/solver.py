@@ -25,9 +25,9 @@ _lib = None
 OPTIMAL, MAX_ITER, NUMERICAL, INFEASIBLE = 0, 1, 2, 3
 STATUS_NAMES = {OPTIMAL: "optimal", MAX_ITER: "maxIterations", NUMERICAL: "error", INFEASIBLE: "infeasible"}
 
-KERNEL_AUTO, KERNEL_BAND, KERNEL_STAGE, KERNEL_STAGE_V1, KERNEL_DENSE = 0, 1, 2, 3, 4
+KERNEL_AUTO, KERNEL_BAND, KERNEL_STAGE, KERNEL_STAGE_V1, KERNEL_DENSE, KERNEL_DENSE_CLUSTER = 0, 1, 2, 3, 4, 5
 
-EXPORTS = ["dsp_lp_template_create", "dsp_lp_template_set_matrix_params", "dsp_lp_template_set_stage_chain1", "dsp_lp_template_create_csr", "dsp_lp_template_create_dense", "dsp_lp_template_create_dense_with_matrix_params", "dsp_lp_analyze_csr", "dsp_lp_template_info", "dsp_lp_template_destroy", "dsp_lp_template_set_stage_wb", "dsp_lp_default_opts", "dsp_lp_solve_batch",
+EXPORTS = ["dsp_lp_template_create", "dsp_lp_template_set_matrix_params", "dsp_lp_template_set_stage_chain1", "dsp_lp_template_create_csr", "dsp_lp_template_create_dense", "dsp_lp_template_create_dense_with_matrix_params", "dsp_lp_template_create_dense_cluster", "dsp_lp_analyze_csr", "dsp_lp_template_info", "dsp_lp_template_destroy", "dsp_lp_template_set_stage_wb", "dsp_lp_default_opts", "dsp_lp_solve_batch",
            "dsp_lp_solve_batch_host", "dsp_lp_launch_count", "dsp_lp_last_launch", "dsp_lp_last_error",
            "dsp_lp_version", "dsp_lp_fp64_peak_tflops"]
 
@@ -90,6 +90,8 @@ def load_library():
     lib.dsp_lp_template_create_dense.restype = C.c_int
     lib.dsp_lp_template_create_dense_with_matrix_params.argtypes = [C.POINTER(_LpDesc), C.c_int32] + [C.c_void_p] * 4 + [C.POINTER(C.c_void_p)]
     lib.dsp_lp_template_create_dense_with_matrix_params.restype = C.c_int
+    lib.dsp_lp_template_create_dense_cluster.argtypes = [C.POINTER(_LpDesc), C.c_int32] + [C.c_void_p] * 4 + [C.POINTER(C.c_void_p)]
+    lib.dsp_lp_template_create_dense_cluster.restype = C.c_int
     lib.dsp_lp_analyze_csr.argtypes = [C.POINTER(_LpDesc)] + [C.POINTER(C.c_int32)] * 4 + [C.c_void_p, C.c_void_p]
     lib.dsp_lp_analyze_csr.restype = C.c_int
     lib.dsp_lp_template_set_matrix_params.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -166,7 +168,9 @@ class BatchLPSolver:
             native_setup = True          # per-problem matrix coefficients need the library's own symbolic setup
         # a template whose A A' is wider than the band kernels take runs on the dense kernel: the library gets the plain LP
         self.dense = kernel == KERNEL_DENSE and t.w > 32
-        if self.dense:
+        # KERNEL_DENSE_CLUSTER: any template (m <= 4096) goes to the dense cluster kernel, with its per-problem matrix if it has one
+        self.cluster = kernel == KERNEL_DENSE_CLUSTER
+        if self.dense or self.cluster:
             native_setup = True
         A = t.A.tocsr(); A.sort_indices()
         Cm = t.Cmap.tocsr(); Bm = t.Bmap.tocsr()
@@ -185,12 +189,12 @@ class BatchLPSolver:
                         b0=p("b0"), bmap=_ParamMap(p("bm_ptr"), p("bm_idx"), p("bm_val")),
                         u0=p("u0"), umap=_ParamMap(p("um_ptr"), p("um_idx"), p("um_val")),
                         o0=float(t.o0), omap=p("omap"), ocmap=p("ocmap"))
-            if self.dense and t.amap is not None:         # per-problem matrix coefficients of a dense template come with its creation
-                create = "dsp_lp_template_create_dense_with_matrix_params"
-                am = [_i32(t.amap[0]), _i32(t.amap[1]), _i32(t.amap[2]), _f64(t.amap[3])]
+            if self.cluster or (self.dense and t.amap is not None):   # per-problem matrix coefficients of a dense template come with its creation
+                create = "dsp_lp_template_create_dense_cluster" if self.cluster else "dsp_lp_template_create_dense_with_matrix_params"
+                am = [_i32(t.amap[k]) for k in range(3)] + [_f64(t.amap[3])] if t.amap is not None else [_i32([0])] * 3 + [_f64([0.0])]
                 keep.update(am=am)
-                rc = self.lib.dsp_lp_template_create_dense_with_matrix_params(C.byref(d), len(am[0]), *(a.ctypes.data_as(C.c_void_p) for a in am),
-                                                                              C.byref(h))
+                cnt = len(am[0]) if t.amap is not None else 0
+                rc = getattr(self.lib, create)(C.byref(d), cnt, *(a.ctypes.data_as(C.c_void_p) for a in am), C.byref(h))
             else:
                 create = "dsp_lp_template_create_dense" if self.dense else "dsp_lp_template_create_csr"
                 rc = getattr(self.lib, create)(C.byref(d), C.byref(h))
@@ -217,7 +221,7 @@ class BatchLPSolver:
             if rc != 0:
                 raise RuntimeError(f"dsp_lp_template_create failed ({rc}): {self.lib.dsp_lp_last_error().decode()}")
         self.handle = h
-        if t.amap is not None and not self.dense:
+        if t.amap is not None and not (self.dense or self.cluster):
             ar, ac, ak, av = _i32(t.amap[0]), _i32(t.amap[1]), _i32(t.amap[2]), _f64(t.amap[3])
             vp_ = lambda a: a.ctypes.data_as(C.c_void_p)
             rc = self.lib.dsp_lp_template_set_matrix_params(h, len(ar), vp_(ar), vp_(ac), vp_(ak), vp_(av))
@@ -232,7 +236,7 @@ class BatchLPSolver:
         self.opts.reg_primal = float(template.meta.get("reg_primal", 1e-8) if reg_primal is None else reg_primal)
         st = t.meta.get("stage_wb")
         self.has_stage = False
-        if st is not None and kernel not in (KERNEL_BAND, KERNEL_DENSE):
+        if st is not None and kernel not in (KERNEL_BAND, KERNEL_DENSE, KERNEL_DENSE_CLUSTER):
             ci, ri = _i32(st["col_idx"]), _i32(st["row_idx"])
             sd = _StageWB(T=st["T"], a=st["a"], binv=st["binv"], half=st["half"], delta=st["delta"], dur=st["dur"],
                           k_rev=st["k_rev"], wcf_off=st["wcf_off"], p_off=st["p_off"],
@@ -241,7 +245,7 @@ class BatchLPSolver:
             self.has_stage = True
         # descriptor-driven stage kernel for templates of the single-storage-chain family (structure found on the template itself)
         self.has_chain1 = False
-        if st is None and kernel not in (KERNEL_BAND, KERNEL_DENSE) and t.m <= 96:
+        if st is None and kernel not in (KERNEL_BAND, KERNEL_DENSE, KERNEL_DENSE_CLUSTER) and t.m <= 96:
             from .lp_template import detect_chain1
             d1 = detect_chain1(t)
             if d1 is not None:

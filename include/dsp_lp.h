@@ -28,7 +28,8 @@
  *
  * Size limits: half bandwidth of A*A' <= 32 (padded to 1,2,4,8,16,32); any m, n -- the per-LP work region lives in shared
  * memory when it fits (up to ~27 000 doubles) and in a device workspace owned by the template handle otherwise.  A wider LP with
- * m <= 1024 goes through dsp_lp_template_create_dense (dense normal equations, below).
+ * m <= 1024 goes through dsp_lp_template_create_dense (dense normal equations, below), one with m <= 4096 through
+ * dsp_lp_template_create_dense_cluster (the same on a thread-block cluster per LP).
  *
  * All pointers in dsp_lp_solve_batch are DEVICE pointers, the call is stream-ordered and does not
  * synchronise.  dsp_lp_solve_batch_host takes HOST pointers and does the copies itself.
@@ -78,7 +79,9 @@ typedef struct {
 enum { DSP_KERNEL_AUTO = 0, DSP_KERNEL_BAND = 1, DSP_KERNEL_STAGE = 2 /* generation 2: several LPs per warp */,
        DSP_KERNEL_STAGE_V1 = 3 /* generation 1: lane per period, T <= 32 (kept as an independent implementation for tests) */,
        DSP_KERNEL_DENSE = 4 /* dense normal equations, one CTA per LP, m <= 1024: what a dense template runs (AUTO picks it there);
-                               on a band template it replaces the band / stage kernels (a cross-check; no per-problem matrices) */ };
+                               on a band template it replaces the band / stage kernels (a cross-check; no per-problem matrices) */,
+       DSP_KERNEL_DENSE_CLUSTER = 5 /* dense normal equations, one thread-block cluster per LP, m <= 4096: what a dense cluster template
+                                       runs (AUTO picks it there); on a band template a cross-check like DSP_KERNEL_DENSE */ };
 
 /* Stage descriptor of the wind+battery price-taker flowsheet (wind_battery_LMP.py:172-267, reduced form):
  * any T (T <= 96: on chip, several LPs per warp; longer, up to the reference's full-year 8736 periods of
@@ -167,6 +170,13 @@ int dsp_lp_template_create_dense(const dsp_lp_desc *desc, dsp_template **out);
  * assembly list into the LP's workspace region (2 nnz + the assembly list's length more doubles per LP in flight). */
 int dsp_lp_template_create_dense_with_matrix_params(const dsp_lp_desc *desc, int32_t count, const int32_t *row, const int32_t *col,
                                                     const int32_t *param, const double *coef, dsp_template **out);
+/* The same hand-over (same rules and messages, count == 0: no per-problem matrix) for m <= 4096 (larger: DSP_E_ARG).  dsp_lp_solve_batch
+ * then runs the dense cluster kernel: one LP per thread-block cluster of 4 CTAs (up to 32 tile rows of 64) or 8, the same iteration
+ * and pivot rule as the dense kernel, a left-looking blocked LDL' and the substitutions split over the cluster's CTAs by tile row.  The
+ * LP's tiles of M (m^2 / 2 doubles, padded to 64) live in the handle's workspace per cluster in flight.  DSP_KERNEL_BAND / _STAGE /
+ * _STAGE_V1 / _DENSE on such a template and dsp_lp_template_set_matrix_params return DSP_E_ARG. */
+int dsp_lp_template_create_dense_cluster(const dsp_lp_desc *desc, int32_t count, const int32_t *row, const int32_t *col,
+                                         const int32_t *param, const double *coef, dsp_template **out);
 /* Per-problem MATRIX coefficients for a template made by dsp_lp_template_create_csr:  A[row][col] = A0[row][col] + sum coef * rparams[param]
  * (row / col in the caller's order; the entry must be in A's pattern).  Needed where a design column is multiplied by per-scenario data --
  * wind system_capacity * capacity_factor[t] with a free wind size, wind_power.py:120-122 + wind_battery_LMP.py:212-216.  The band kernel then
@@ -200,7 +210,8 @@ int dsp_lp_solve_batch_host(dsp_template *t, int64_t N,
                             const dsp_opts *opts,
                             double *obj, int32_t *status, int32_t *iters, double *x, double *y);
 
-/* Introspection used by tests / bench: kernel launches issued so far, last launch geometry. */
+/* Introspection used by tests / bench: kernel launches issued so far, last launch geometry (grid in CTAs, block, dynamic shared
+ * memory; problems_per_cta: LPs per CTA, or for the dense cluster kernel the cluster size in CTAs). */
 int64_t dsp_lp_launch_count(void);
 int dsp_lp_last_launch(int32_t *grid, int32_t *block, int32_t *smem_bytes, int32_t *problems_per_cta);
 const char *dsp_lp_last_error(void);
