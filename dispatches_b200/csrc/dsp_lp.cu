@@ -15,6 +15,8 @@
 //   * Mehrotra predictor-corrector; M is factorised once per iteration by a band LDL' (half bandwidth w),
 //     two band solves per iteration.  The numpy mirror of exactly this algorithm is oracle/ipm_numpy.py.
 //
+// Kernel `dsp_ipm_band_split_kernel` (DSP_KERNEL_BAND_SPLIT, band templates, w <= 8, m >= 64 w): the band kernel's iteration, one warp
+// per LP with the rows cut into 32 chunks over its lanes and a partitioned band LDL' (dsp_band_split.cuh), state in a workspace.
 // Kernel `dsp_ipm_dense_kernel` (any bandwidth, m <= 1024; dsp_lp_template_create_dense or DSP_KERNEL_DENSE): the same iteration,
 // one CTA per LP, M = A D A' dense in a workspace, blocked LDL' with FP64 tensor-core trailing updates (dsp_dense.cuh).
 // Kernel `dsp_ipm_dense_cluster_kernel` (m <= 4096; dsp_lp_template_create_dense_cluster or DSP_KERNEL_DENSE_CLUSTER): the same, one
@@ -493,6 +495,8 @@ __global__ void __launch_bounds__(kMaxWarps * 32, 1) dsp_ipm_band_kernel(const K
         if (st != DSP_OPTIMAL) solve_one<BW>(W, H, P, (long long)t, lane, 0.99, 10.0 * P.reg, it0, &st, &it0);
     }
 }
+
+#include "dsp_band_split.cuh"
 
 }  // namespace
 
@@ -1171,6 +1175,13 @@ struct dsp_template {
         const double *am_coef;
     };
     mutable Dense dn;
+    struct Split {                 // the split band kernel's renumbered template (built at the first DSP_KERNEL_BAND_SPLIT call)
+        bool ready;
+        int Sr, Sc;
+        const int *ccnt, *cnat, *A_ptr, *A_idx, *At_ptr, *At_idx, *asm_ptr, *asm_col;
+        const double *A_val, *At_val, *asm_val;
+    };
+    mutable Split spl;
 };
 
 namespace {
@@ -1193,6 +1204,17 @@ BandKernel band_kernel(int w, bool ws, bool hot_in_smem) {
         case 8: return band_kernel_w<8>(ws, hot_in_smem);
         case 16: return band_kernel_w<16>(ws, hot_in_smem);
         default: return band_kernel_w<32>(ws, hot_in_smem);
+    }
+}
+
+// split band kernel for half bandwidth W <= 8 (ensure_split refuses 16 and 32: those instantiations spill)
+using BandSplitKernel = void (*)(KParams, SplitParams);
+BandSplitKernel band_split_kernel(int w) {
+    switch (w) {
+        case 1: return dsp_ipm_band_split_kernel<1>;
+        case 2: return dsp_ipm_band_split_kernel<2>;
+        case 4: return dsp_ipm_band_split_kernel<4>;
+        default: return dsp_ipm_band_split_kernel<8>;
     }
 }
 
@@ -1248,6 +1270,7 @@ int template_init(dsp_template *T, const dsp_template_desc *D) {
     T->dense_only = false;
     T->cluster_only = false;
     memset(&T->dn, 0, sizeof(T->dn));
+    memset(&T->spl, 0, sizeof(T->spl));
     CK(cudaGetDevice(&T->device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, T->device));
@@ -1809,6 +1832,146 @@ static int launch_band(const dsp_template *T, KParams K, cudaStream_t st) {
     return launched(ctas, warps * 32, smem, warps);
 }
 
+// the split band kernel's data of a band template (dsp_band_split.cuh), built from its device copy of A and of the band assembly list
+// at the first DSP_KERNEL_BAND_SPLIT call: rows cut into 32 chunks, a column on the lane of the first row it appears in, the CSR, CSC
+// and assembly list renumbered to split rows / columns
+static int ensure_split(const dsp_template *T) {
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lk(mu);
+    const KParams &K = T->kp;
+    const int W = K.w, m = K.m, n = K.n, nnz = K.nnz, nasm = K.nasm;
+    if (K.n_amap > 0) {
+        g_err = "dsp_lp_solve_batch: DSP_KERNEL_BAND_SPLIT does not take per-problem matrix coefficients (dsp_lp_template_set_matrix_params); "
+                "use DSP_KERNEL_BAND";
+        return DSP_E_ARG;
+    }
+    if (W > 8) {
+        g_err = "dsp_lp_solve_batch: DSP_KERNEL_BAND_SPLIT takes half bandwidths up to 8 (w = " + std::to_string(W) + "); use DSP_KERNEL_BAND";
+        return DSP_E_ARG;
+    }
+    if (m < 64 * W) {
+        g_err = "dsp_lp_solve_batch: DSP_KERNEL_BAND_SPLIT needs m >= 64 w, two separator widths per row chunk (m = " + std::to_string(m) +
+                ", w = " + std::to_string(W) + ")";
+        return DSP_E_ARG;
+    }
+    if (T->spl.ready) return 0;
+    std::vector<unsigned char> hot(K.hot_bytes);
+    CK(cudaMemcpy(hot.data(), K.hot_g, hot.size(), cudaMemcpyDeviceToHost));
+    const double *A_val = (const double *)hot.data(), *asm_val = A_val + 2 * (size_t)nnz;
+    const int *A_ptr = (const int *)(asm_val + nasm), *A_idx = A_ptr + m + 1, *At_ptr = A_idx + nnz, *At_idx = At_ptr + n + 1;
+    const int *asm_ptr = At_idx + nnz, *asm_col = asm_ptr + m * (W + 1) + 1;
+    const double *At_val = A_val + nnz;
+    const int base = m / 32, rem = m % 32, Sr = base + (rem > 0);
+    auto r0 = [&](int L) { return L * base + std::min(L, rem); };
+    std::vector<int> rlane(m), rsplit(m);
+    for (int L = 0; L < 32; ++L)
+        for (int r = r0(L); r < r0(L + 1); ++r) { rlane[r] = L; rsplit[r] = (r - r0(L)) * 32 + L; }
+    std::vector<int> owner(n, -1);
+    for (int r = 0; r < m; ++r)
+        for (int q = A_ptr[r]; q < A_ptr[r + 1]; ++q)
+            if (owner[A_idx[q]] < 0) owner[A_idx[q]] = rlane[r];
+    std::vector<int> ccnt(32, 0), csplit(n);
+    for (int c = 0; c < n; ++c) {
+        const int L = std::max(owner[c], 0);       // a column in no row: lane 0
+        csplit[c] = ccnt[L]++ * 32 + L;
+    }
+    const int Sc = *std::max_element(ccnt.begin(), ccnt.end());
+    std::vector<int> cnat((size_t)Sc * 32, -1);
+    for (int c = 0; c < n; ++c) cnat[csplit[c]] = c;
+    std::vector<int> sA_ptr((size_t)Sr * 32 + 1, 0), sA_idx, sAt_ptr((size_t)Sc * 32 + 1, 0), sAt_idx, sasm_ptr((size_t)(W + 1) * Sr * 32 + 1, 0), sasm_col;
+    std::vector<double> sA_val, sAt_val, sasm_val;
+    std::vector<int> rnat((size_t)Sr * 32, -1);
+    for (int r = 0; r < m; ++r) rnat[rsplit[r]] = r;
+    for (size_t i = 0; i < rnat.size(); ++i) {
+        if (const int r = rnat[i]; r >= 0)
+            for (int q = A_ptr[r]; q < A_ptr[r + 1]; ++q) { sA_idx.push_back(csplit[A_idx[q]]); sA_val.push_back(A_val[q]); }
+        sA_ptr[i + 1] = (int)sA_idx.size();
+    }
+    for (size_t j = 0; j < cnat.size(); ++j) {
+        if (const int c = cnat[j]; c >= 0)
+            for (int q = At_ptr[c]; q < At_ptr[c + 1]; ++q) { sAt_idx.push_back(rsplit[At_idx[q]]); sAt_val.push_back(At_val[q]); }
+        sAt_ptr[j + 1] = (int)sAt_idx.size();
+    }
+    for (int k = 0; k <= W; ++k)
+        for (size_t i = 0; i < rnat.size(); ++i) {
+            const size_t e = (size_t)k * Sr * 32 + i;
+            if (const int r = rnat[i]; r >= 0)
+                for (int q = asm_ptr[r * (W + 1) + k]; q < asm_ptr[r * (W + 1) + k + 1]; ++q) {
+                    sasm_col.push_back(csplit[asm_col[q]]);
+                    sasm_val.push_back(asm_val[q]);
+                }
+            sasm_ptr[e + 1] = (int)sasm_col.size();
+        }
+    dsp_template *Tm = const_cast<dsp_template *>(T);
+    dsp_template::Split &D = Tm->spl;
+    auto up_i = [&](const std::vector<int> &v, const int **dst) -> int {
+        int *d;
+        if (int rc = upload(v, &d)) return rc;
+        Tm->dev_allocs.push_back(d);
+        *dst = d;
+        return 0;
+    };
+    auto up_d = [&](const std::vector<double> &v, const double **dst) -> int {
+        double *d;
+        if (int rc = upload(v, &d)) return rc;
+        Tm->dev_allocs.push_back(d);
+        *dst = d;
+        return 0;
+    };
+    int rc = up_i(ccnt, &D.ccnt);
+    if (!rc) rc = up_i(cnat, &D.cnat);
+    if (!rc) rc = up_i(sA_ptr, &D.A_ptr);
+    if (!rc) rc = up_i(sA_idx, &D.A_idx);
+    if (!rc) rc = up_d(sA_val, &D.A_val);
+    if (!rc) rc = up_i(sAt_ptr, &D.At_ptr);
+    if (!rc) rc = up_i(sAt_idx, &D.At_idx);
+    if (!rc) rc = up_d(sAt_val, &D.At_val);
+    if (!rc) rc = up_i(sasm_ptr, &D.asm_ptr);
+    if (!rc) rc = up_i(sasm_col, &D.asm_col);
+    if (!rc) rc = up_d(sasm_val, &D.asm_val);
+    if (rc) return rc;
+    D.Sr = Sr; D.Sc = Sc;
+    D.ready = true;
+    return 0;
+}
+
+// split band kernel: one warp per LP, kSplitWarps warps per CTA, as many CTAs as are co-resident (spread one warp per CTA while there
+// are fewer LPs than SMs x kSplitWarps); every warp's region in the handle's workspace.  The band kernel follows in retry mode.
+static int launch_band_split(const dsp_template *T, KParams K, cudaStream_t st) {
+    int rc = ensure_split(T);
+    if (rc) return rc;
+    const dsp_template::Split &D = T->spl;
+    SplitParams S;
+    S.Sr = D.Sr; S.Sc = D.Sc; S.ccnt = D.ccnt; S.cnat = D.cnat;
+    S.A_ptr = D.A_ptr; S.A_idx = D.A_idx; S.A_val = D.A_val; S.At_ptr = D.At_ptr; S.At_idx = D.At_idx; S.At_val = D.At_val;
+    S.asm_ptr = D.asm_ptr; S.asm_col = D.asm_col; S.asm_val = D.asm_val;
+    const int W = K.w;
+    S.warp_doubles = (split_vec_doubles(D.Sr, D.Sc) + (long long)(2 * W + 1) * D.Sr * 32 + W * W * 32 + W * W + W + 31) / 32 * 32;
+    const size_t per_warp = (size_t)S.warp_doubles * sizeof(double);
+    const BandSplitKernel kern = band_split_kernel(W);
+    int occ = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32 * kSplitWarps, 0));
+    long long warps = std::min<long long>(K.N, (long long)T->sm_count * std::max(occ, 1) * kSplitWarps);
+    while (warps > 1 && (size_t)warps * per_warp > T->ws_cap) warps /= 2;
+    const int wpb = (int)std::min<long long>(kSplitWarps, std::max<long long>(1, warps / T->sm_count));
+    const long long blocks = (warps + wpb - 1) / wpb;
+    rc = grow_ws(T, (size_t)blocks * wpb * per_warp, st);
+    if (rc) return rc;
+    S.ws = T->ws;
+    CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
+    kern<<<(unsigned)blocks, 32 * wpb, 0, st>>>(K, S);
+    rc = launched(blocks, 32 * wpb, 0, wpb);
+    if (rc) return rc;
+    // the LPs the split kernel leaves MAX_ITER / NUMERICAL get the band kernel's sequential elimination order (as behind the
+    // long-horizon stage kernel)
+    K.retry_only = 1;
+    rc = launch_band(T, K, st);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(g_mu);          // dsp_lp_last_launch reports the split kernel's geometry
+    g_last_grid = (int)blocks; g_last_block = 32 * wpb; g_last_smem = 0; g_last_ppc = wpb;
+    return 0;
+}
+
 // the dense kernels' data of a band template, built from its device copy of A at the first DSP_KERNEL_DENSE or _DENSE_CLUSTER call
 static int ensure_dense(const dsp_template *T, bool cluster) {
     static std::mutex mu;
@@ -1948,6 +2111,7 @@ static int launch_batch(const dsp_template *T, int64_t N, const double *cparams,
         if (rc) return rc;
         return launch_dense(T, K, st);
     }
+    if (o.kernel == DSP_KERNEL_BAND_SPLIT) return launch_band_split(T, K, st);
     const bool stage = o.kernel == DSP_KERNEL_AUTO || o.kernel == DSP_KERNEL_STAGE;
     if (T->has_stage && T->sp.T > kStage2MaxT && stage) {
         const int rc = launch_stage2_long(T, K, st);

@@ -27,13 +27,16 @@ from .solver import KERNEL_DENSE, KERNEL_DENSE_CLUSTER, BatchLPSolver, OPTIMAL, 
 _SOLVERS = {}
 
 
-def get_solver(kind, T, **kw) -> BatchLPSolver:
+def get_solver(kind, T, kernel=None, **kw) -> BatchLPSolver:
+    """the cached solver of a (flowsheet, T, options) template; kernel: a solver.KERNEL_* choice (None: the library's default)"""
     key = (kind, T, tuple(sorted(kw.items())))
+    if kernel is not None:
+        key = key + (("kernel", kernel),)
     if key not in _SOLVERS:
         builder = dict(wind_battery=TP.wind_battery, wind_battery_design=TP.wind_battery_design,
                        wind_battery_pem=TP.wind_battery_pem, nuclear=TP.nuclear,
                        fossil_surrogate=TP.fossil_surrogate)[kind]
-        _SOLVERS[key] = BatchLPSolver(builder(T, **kw))
+        _SOLVERS[key] = BatchLPSolver(builder(T, **kw)) if kernel is None else BatchLPSolver(builder(T, **kw), kernel=kernel)
     return _SOLVERS[key]
 
 
@@ -114,14 +117,16 @@ def _lmps(input_params, T):
     return np.ascontiguousarray(lmp)
 
 
-def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solution=True):
+def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solution=True, kernel=None):
+    """kernel: a solver.KERNEL_* choice for the band-template paths (None: the library's default, e.g. KERNEL_BAND_SPLIT for a long
+    horizon on the split band kernel); the free-wind design (per-problem matrix coefficients) does not take it"""
     T = int(n_time_points)
     design = bool(input_params.get("design_opt", False))
     lmp = _lmps(input_params, T)
     cf = _capacity_factors(input_params, T)
     if design and not input_params.get("extant_wind", True):
         return _wind_battery_free_wind(T, lmp, cf, input_params, verbose)
-    sol = get_solver("wind_battery_design" if design else "wind_battery", T,
+    sol = get_solver("wind_battery_design" if design else "wind_battery", T, kernel=kernel,
                      extant_wind=bool(input_params.get("extant_wind", True)))
     want_solution = want_solution or design          # the optimal battery size is read from the solution
     rp = TP.wind_battery_rparams(T, cf, input_params["wind_mw"], input_params["batt_mw"])
@@ -176,7 +181,8 @@ def _wind_battery_free_wind(T, lmp, cf, input_params, verbose):
     return PriceTakerResult("wind_battery", T, lmp, r.obj, r.status, r.iters, xm, names, sizes)
 
 
-def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_solution=True):
+def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_solution=True, kernel=None):
+    """kernel: a solver.KERNEL_* choice (None: the library's default)"""
     mode = input_params.get("design_opt", False)
     if mode not in (False, "PEM") or (mode == "PEM" and not input_params.get("extant_wind", True)):
         raise NotImplementedError("only design_opt False and \"PEM\" (extant wind) are on the batched GPU path")
@@ -188,7 +194,7 @@ def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_sol
     batt = np.zeros(1) if pem_design else np.asarray(input_params["batt_mw"], float)   # "PEM" fixes the battery at 0 (:228)
     with_batt = bool(np.any(batt > 0))
     want_solution = want_solution or pem_design
-    sol = get_solver("wind_battery_pem", T, with_battery=with_batt, extant_wind=bool(input_params.get("extant_wind", True)),
+    sol = get_solver("wind_battery_pem", T, kernel=kernel, with_battery=with_batt, extant_wind=bool(input_params.get("extant_wind", True)),
                      pem_design=pem_design)
     rp = TP.wind_battery_rparams(T, cf, input_params["wind_mw"], batt, pem_mw=input_params["pem_mw"])
     if rp.shape[0] == 1:
@@ -207,10 +213,11 @@ def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_sol
     return PriceTakerResult("wind_battery_pem", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes)
 
 
-def nuclear_dispatch_optimize(n_time_points, lmps, want_solution=False, **flowsheet_options):
+def nuclear_dispatch_optimize(n_time_points, lmps, want_solution=False, kernel=None, **flowsheet_options):
+    """kernel: a solver.KERNEL_* choice (None: the library's default)"""
     T = int(n_time_points)
     lmp = np.ascontiguousarray(np.atleast_2d(np.asarray(lmps, float))[:, :T])
-    sol = get_solver("nuclear", T, **flowsheet_options)
+    sol = get_solver("nuclear", T, kernel=kernel, **flowsheet_options)
     r = sol.solve_host(lmp, None, want_x=want_solution)
     return PriceTakerResult("nuclear", T, lmp, r.obj, r.status, r.iters,
                             sol.to_model_space(r.x) if want_solution else None, sol.t.col_names, {})

@@ -131,7 +131,9 @@ class B200IPM:
     def solve(self, model, tee=False, batch_params=None, options=None, **_):
         opts = dict(self.options); opts.update(options or {})
         t, vars_, cons, p0 = walk_model(model, batch_params=list((batch_params or {}).keys()))
-        sol = BatchLPSolver(t, tol=opts["tol"], feas_tol=opts["feas_tol"], max_iter=opts["max_iter"], native_setup=True)
+        # options["kernel"]: a solver.KERNEL_* choice, e.g. KERNEL_BAND_SPLIT for a long horizon (unset: the library's default)
+        kern = {"kernel": int(opts["kernel"])} if opts.get("kernel") is not None else {}
+        sol = BatchLPSolver(t, tol=opts["tol"], feas_tol=opts["feas_tol"], max_iter=opts["max_iter"], native_setup=True, **kern)
         if batch_params:
             pv = np.column_stack([np.asarray(batch_params[p], float) for p in batch_params])
         else:

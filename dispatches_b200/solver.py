@@ -25,7 +25,7 @@ _lib = None
 OPTIMAL, MAX_ITER, NUMERICAL, INFEASIBLE = 0, 1, 2, 3
 STATUS_NAMES = {OPTIMAL: "optimal", MAX_ITER: "maxIterations", NUMERICAL: "error", INFEASIBLE: "infeasible"}
 
-KERNEL_AUTO, KERNEL_BAND, KERNEL_STAGE, KERNEL_STAGE_V1, KERNEL_DENSE, KERNEL_DENSE_CLUSTER = 0, 1, 2, 3, 4, 5
+KERNEL_AUTO, KERNEL_BAND, KERNEL_STAGE, KERNEL_STAGE_V1, KERNEL_DENSE, KERNEL_DENSE_CLUSTER, KERNEL_BAND_SPLIT = 0, 1, 2, 3, 4, 5, 6
 
 EXPORTS = ["dsp_lp_template_create", "dsp_lp_template_set_matrix_params", "dsp_lp_template_set_stage_chain1", "dsp_lp_template_create_csr", "dsp_lp_template_create_dense", "dsp_lp_template_create_dense_with_matrix_params", "dsp_lp_template_create_dense_cluster", "dsp_lp_analyze_csr", "dsp_lp_template_info", "dsp_lp_template_destroy", "dsp_lp_template_set_stage_wb", "dsp_lp_default_opts", "dsp_lp_solve_batch",
            "dsp_lp_solve_batch_host", "dsp_lp_launch_count", "dsp_lp_last_launch", "dsp_lp_last_error",

@@ -81,7 +81,14 @@ enum { DSP_KERNEL_AUTO = 0, DSP_KERNEL_BAND = 1, DSP_KERNEL_STAGE = 2 /* generat
        DSP_KERNEL_DENSE = 4 /* dense normal equations, one CTA per LP, m <= 1024: what a dense template runs (AUTO picks it there);
                                on a band template it replaces the band / stage kernels (a cross-check; no per-problem matrices) */,
        DSP_KERNEL_DENSE_CLUSTER = 5 /* dense normal equations, one thread-block cluster per LP, m <= 4096: what a dense cluster template
-                                       runs (AUTO picks it there); on a band template a cross-check like DSP_KERNEL_DENSE */ };
+                                       runs (AUTO picks it there); on a band template a cross-check like DSP_KERNEL_DENSE */,
+       DSP_KERNEL_BAND_SPLIT = 6 /* band template, the horizon split over the warp: one warp per LP, rows cut into 32 chunks, a
+                                    partitioned (nested-dissection) band LDL' (csrc/dsp_band_split.cuh); the band kernel's iteration and
+                                    status rules.  The band kernel follows on the same stream and re-solves only the LPs it leaves
+                                    MAX_ITER / NUMERICAL (two launches).  Needs w <= 8 (w: the half bandwidth rounded up to 1, 2, 4 or
+                                    8), m >= 64 w and a template without per-problem matrix coefficients; dense templates are refused;
+                                    a stage descriptor is ignored, as with DSP_KERNEL_BAND.  dsp_lp_last_launch reports the split
+                                    kernel's grid.  Not chosen by DSP_KERNEL_AUTO. */ };
 
 /* Stage descriptor of the wind+battery price-taker flowsheet (wind_battery_LMP.py:172-267, reduced form):
  * any T (T <= 96: on chip, several LPs per warp; longer, up to the reference's full-year 8736 periods of
