@@ -1,12 +1,12 @@
 """All 10 000 C2 LPs and the strided C5 sample (tests/real_lps.py) on the GPU through check_exact's measures, on their usual kernel
-(stage 2) and on the dense kernel (DSP_KERNEL_DENSE), and the PV + battery + hydrogen design LPs (baked and with a PV series per LP,
-T = 24 and 48) on the dense kernel: prints, per run, how many LPs ended OPTIMAL and the largest error of every measure, and exits
-non-zero if any LP is not OPTIMAL or over a bar.
+(stage 2) and on the dense kernel (DSP_KERNEL_DENSE), the PV + battery + hydrogen design LPs (baked and with a PV series per LP)
+at T = 24 and 48 on the dense kernel and the dense cluster kernel, and at T = 72, 96 and 168 on the dense cluster kernel: prints, per
+run, how many LPs ended OPTIMAL and the largest error of every measure, and exits non-zero if any LP is not OPTIMAL or over a bar.
 
     python tests/checks/gpu_exact_real.py [--procs P]
 
-Exact certification (about 7 ms per 24-hour dispatch LP and 0.2 to 2 s per design LP on one core) and the per-LP KKT residuals run
-in P worker processes."""
+Exact certification (about 7 ms per 24-hour dispatch LP, and on one core 0.2 to 2 s per design LP at T = 24 and 48, 2 to 6 s at
+T = 72, about 30 s at T = 96 and 40 to 80 s at T = 168) and the per-LP KKT residuals run in P worker processes."""
 import argparse
 import multiprocessing as mp
 import sys
@@ -43,9 +43,10 @@ def _sets(procs):
 
     yield "C2", c2, (S.KERNEL_AUTO, S.KERNEL_DENSE)
     yield "C5", c5, (S.KERNEL_AUTO,)
-    for T, N in ((24, 256), (48, 64)):
-        yield f"solar_design{T}", lambda T=T, N=N: R.solar_design(T, N, procs=procs), (S.KERNEL_DENSE,)
-        yield f"solar_design_pv{T}", lambda T=T, N=N: R.solar_design_pv(T, N, procs=procs), (S.KERNEL_DENSE,)
+    for T, N in ((24, 256), (48, 64), (72, 64), (96, 32), (168, 12)):
+        kernels = (S.KERNEL_DENSE, S.KERNEL_DENSE_CLUSTER) if 15 * T + 3 <= 1024 else (S.KERNEL_DENSE_CLUSTER,)
+        yield f"solar_design{T}", lambda T=T, N=N: R.solar_design(T, N, procs=procs), kernels
+        yield f"solar_design_pv{T}", lambda T=T, N=N: R.solar_design_pv(T, N, procs=procs), kernels
 
 
 def main():
@@ -58,7 +59,8 @@ def main():
         s = make()
         t1 = time.perf_counter()
         for kernel in kernels:
-            name = set_name + (" on the dense kernel" if kernel == S.KERNEL_DENSE else "")
+            name = set_name + {S.KERNEL_DENSE: " on the dense kernel",
+                               S.KERNEL_DENSE_CLUSTER: " on the dense cluster kernel"}.get(kernel, "")
             bad += _check(name, s, S.BatchLPSolver(s.t, kernel=kernel), a.procs, t1 - t0)
     return 1 if bad else 0
 

@@ -11,11 +11,11 @@ degenerate vertices: the dispatch LPs have zero prices, idle empty batteries and
 strictly inside their bounds at almost every optimum.  A degenerate vertex is certified from HiGHS' basis or from an exact repair of
 it: HiGHS solves in floating point (and drops entries below its small-matrix-value threshold, such as the 1.2e-16 of sin(pi) in a
 PV series), so its basis can be primal infeasible in exact arithmetic by 1e-14 or so; a bounded dual simplex in exact arithmetic
-(_repair) then pivots it to a basis that verifies.  Everything is verified against the LP as the kernels receive it, tiny entries
-included.  The answer is the optimum of that very LP, not another solver's approximation of it; when the basis does not verify, it
-raises (there is no fall-back to the floating-point answer).  The optimum
-is unique in x when every nonbasic reduced cost is nonzero, and unique in y when every basic column lies strictly inside its bounds
-(and no row slack is basic).  Either way, ``fixed`` marks the columns every optimal x has at the bound x* sits at (r*_j != 0,
+(_repair) then pivots it to a basis that verifies (up to about 100 pivots on the week-long design LPs, within max_pivots(m)).
+Everything is verified against the LP as the kernels receive it, tiny entries included.  The answer is the optimum of that very LP,
+not another solver's approximation of it; when the basis does not verify, it raises (there is no fall-back to the floating-point
+answer).  The optimum is unique in x when every nonbasic reduced cost is nonzero, and unique in y when every basic column lies
+strictly inside its bounds (and no row slack is basic).  Either way, ``fixed`` marks the columns every optimal x has at the bound x* sits at (r*_j != 0,
 complementary slackness with y*) and ``inside`` the columns at which every optimal y has a zero reduced cost (0 < x*_j < u_j).
 
 ``kkt_residuals`` measures any (x, y) a kernel returns -- degenerate LPs included -- against the same LP: primal residual, bound
@@ -51,6 +51,7 @@ class ExactOptimum:
     fixed: np.ndarray = None   # [n] bool, r*_j != 0: every optimal x has x_j at the bound x*_j sits at
     inside: np.ndarray = None  # [n] bool, 0 < x*_j < u_j: every optimal y has r_j(y) = 0
     pivots: int = 0            # dual simplex pivots that repaired HiGHS' basis (0: it verified as it is)
+    basis: tuple = None        # (col [n] int8, row_basic [m] bool) of the verified basis, as highs_basis returns it and basis= takes it
 
 
 def _fr(v):
@@ -200,8 +201,15 @@ def _primal_violations(xF, sF, col, uF):
     return out
 
 
-MAX_PIVOTS = 64          # the repair's pivot limit (the 48-hour design LPs need up to 48: one pivot per row left off by HiGHS)
 REPAIR_GATE = 1e-8       # the repair starts only where every exact infeasibility is at most this, relative to the primal scale
+
+
+def max_pivots(m):
+    """the repair's pivot limit for an LP of m rows.  The pivots a repair needs grow with the LP: the 48-hour design LPs (m = 723)
+    need up to 48, the 96-hour ones (m = 1 443) about 95 and the week-long ones (m = 2 523) about 100.  A limit of m / 8, and never
+    below 64, keeps a wide margin over that and still stops a repair that does not converge.  The limit only decides when a repair
+    gives up: a repair that succeeds takes the same pivots under any limit above its count."""
+    return max(64, m // 8)
 
 
 def _repair(cols, cF, bF, uF, col, row_basic, vertex, scale):
@@ -211,12 +219,13 @@ def _repair(cols, cF, bF, uF, col, row_basic, vertex, scale):
     Leaving: the most infeasible basic variable (lowest index on ties).  Entering: the ratio test |r_j / alpha_j| over the nonbasic
     columns that move it towards its bound, Bland's rule (lowest index) on ties.  After each pivot the basic solution is solved
     again from scratch.  A basis that is also dual infeasible is not repaired (the LPs here never need a primal simplex leg): it
-    raises, as does a ratio test with no candidate (the LP is infeasible in exact arithmetic) or MAX_PIVOTS pivots without a
+    raises, as does a ratio test with no candidate (the LP is infeasible in exact arithmetic) or max_pivots(m) pivots without a
     feasible basis.  Returns (col, row_basic, vertex, pivots)."""
     m, n = len(bF), len(cF)
     col, row_basic = col.copy(), row_basic.copy()
     fixed = np.array([u is not None and u == 0 for u in uF])
-    for pivots in range(MAX_PIVOTS + 1):
+    cap = max_pivots(m)
+    for pivots in range(cap + 1):
         xF, sF, yF, rF = vertex
         viol = _primal_violations(xF, sF, col, uF)
         if not viol:
@@ -228,7 +237,7 @@ def _repair(cols, cF, bF, uF, col, row_basic, vertex, scale):
                                    f"too far to repair")
             if any(not fixed[j] and ((col[j] == 0 and rF[j] < 0) or (col[j] == 2 and rF[j] > 0)) for j in range(n)):
                 raise NotCertified("HiGHS' basis is primal and dual infeasible")
-        elif pivots == MAX_PIVOTS:
+        elif pivots == cap:
             break
         p = min(viol, key=lambda v: (-abs(viol[v]), v))
         bidx, sidx = np.flatnonzero(col == 1), np.flatnonzero(row_basic)
@@ -255,7 +264,7 @@ def _repair(cols, cF, bF, uF, col, row_basic, vertex, scale):
         else:
             row_basic[p - n] = False
         vertex = _vertex(cols, cF, bF, uF, col, row_basic)
-    raise NotCertified(f"HiGHS' basis not repaired in {MAX_PIVOTS} pivots")
+    raise NotCertified(f"HiGHS' basis not repaired in {cap} pivots")
 
 
 def exact_optimum(t, cparams_row, rparams_row, basis=None) -> ExactOptimum:
@@ -319,7 +328,8 @@ def exact_optimum(t, cparams_row, rparams_row, basis=None) -> ExactOptimum:
                         x_margin=float(min(inside, default=math.inf)) / max(1.0, float(np.abs(x).max(initial=0.0))),
                         r_margin=float(min((abs(rF[j]) for j in range(n) if not basic[j]), default=math.inf)) / sc,
                         r=np.array([float(v) for v in rF]), fixed=np.array([v != 0 for v in rF]),
-                        inside=np.array([xF[j] > 0 and (not fin[j] or xF[j] < uF[j]) for j in range(n)]), pivots=pivots)
+                        inside=np.array([xF[j] > 0 and (not fin[j] or xF[j] < uF[j]) for j in range(n)]), pivots=pivots,
+                        basis=(col, row_basic))
 
 
 def kkt_residuals(t, cparams_row, rparams_row, x, y, lp_zero=False):

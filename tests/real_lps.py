@@ -6,9 +6,10 @@ for them.  Each set here is built deterministically from the committed price / c
 the scenario batches of dispatches_b200/scenarios.py, certified LP by LP with exact_lp.exact_optimum (HiGHS' final basis,
 verified in exact arithmetic, or its exact repair) and cached per process.  The sets cover the wind + battery dispatch (C2, C5,
 real windows of 2 to 256 hours, the edges), nuclear, fossil, wind + battery + PEM, the double-loop operation LPs, battery design,
-and PV + battery + hydrogen at fixed sizes and in design (one PV series baked into A, or one per LP as matrix coefficients).  Not
-covered: the free-wind design, which HiGHS reports unbounded at 1e-10 tolerances, and the full-year LP, whose exact certification
-takes over a minute.
+and PV + battery + hydrogen at fixed sizes and in design (one PV series baked into A, or one per LP as matrix coefficients) over
+24 hours to a week (m = 363 to 2 523; a week-long design LP takes about 70 s on one core, so the long sets take ``procs``).  Not
+covered: the free-wind design, which HiGHS reports unbounded at 1e-10 tolerances, and the full-year LPs, whose exact certification
+would take far longer.
 
 ``check_exact`` measures a kernel's answer on such a set against what every optimum of the LP shares: the objective, the KKT
 conditions, x / y element-wise where they are unique, and on every LP the columns every optimal x has at a bound (``fixed``)
@@ -58,6 +59,8 @@ class ExactSet:
     x_margin: np.ndarray       # [N] ExactOptimum.x_margin
     r_margin: np.ndarray       # [N] ExactOptimum.r_margin
     pivots: np.ndarray         # [N] ExactOptimum.pivots: exact dual simplex pivots that repaired HiGHS' basis
+    col: np.ndarray            # [N, n] int8 and
+    row_basic: np.ndarray      # [N, m] bool: the verified basis of each LP (ExactOptimum.basis)
 
     def __len__(self):
         return len(self.obj)
@@ -93,7 +96,7 @@ def certify(t, cparams, rparams, procs=1):
     st = lambda f: np.array([getattr(e, f) for e in es])
     return ExactSet(t, cparams, rparams, st("x"), st("y"), st("r"), st("obj"), st("lp_mag"), st("fixed"), st("inside"),
                     st("unique_x"), st("unique_y"), np.array([o[1] for o in out]), np.array([o[2] for o in out]), st("x_margin"),
-                    st("r_margin"), st("pivots"))
+                    st("r_margin"), st("pivots"), np.array([e.basis[0] for e in es]), np.array([e.basis[1] for e in es]))
 
 
 # ---------------------------------------------------------------------------------------------------------------------

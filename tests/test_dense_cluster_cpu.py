@@ -1,7 +1,7 @@
 """The dense cluster kernel's algorithm on the CPU: its cluster factorisation and substitutions (csrc/dsp_dense.cuh, cluster_column /
 cluster_panel / cluster_fwd / cluster_bwd) on the SIMT emulator with the ranks run one after another between the cluster barriers,
 against the single-CTA routines (bit for bit) and numpy, including zero and negative pivots and m not a multiple of the tile; the
-ranks' tile ownership; the numpy mirror on the design LP past the old 1024-row limit against HiGHS; and the C ABI's argument checks of
+ranks' tile ownership; the numpy mirror on the design LP past the old 1024-row limit against its exact optima; and the C ABI's argument checks of
 dsp_lp_template_create_dense_cluster, which come before any CUDA call."""
 import ctypes as C
 import shutil
@@ -11,9 +11,10 @@ from pathlib import Path
 import numpy as np
 import pytest
 
-from dispatches_b200 import solver as S, templates as TP
-from oracle import highs as H, ipm_dense_numpy as ID, lp_models as L
-from test_dense_mirror import PAR, _design_batch
+import real_lps as R
+from dispatches_b200 import solver as S
+from oracle import ipm_dense_numpy as ID
+from oracle.highs import host_cores
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent
@@ -107,31 +108,29 @@ def test_ranks_own_every_target_tile_once(emu, nt, csize):
         assert sorted(seen) == list(range(J, nt))
 
 
+# LPs of the certified design sets the mirror runs: the reference's case and two perturbed ones baked; an exact-zero quarter, an
+# all-zero PV series and cf = 1 hours with a PV series per LP
+MIRROR_LPS = {False: [0, 1, 2], True: [R.SOLAR_PV.index(c) for c in ("zero_hours", "all_zero", "cf_one")]}
+
+
 @pytest.mark.parametrize("T", [72, 96])
 def test_mirror_solves_the_design_lp_past_1024_rows(T):
     """the numpy mirror of the dense kernels' iteration on the design LP with m = 15 T + 3 > 1024 rows, baked and with a PV series per
-    LP: all OPTIMAL, within 1e-8 of HiGHS"""
-    N = 2
-    lmp, load, cfs = _design_batch(T, N, 3)
-    t = TP.solar_battery_hydrogen_design(T, cfs, **PAR)
-    assert 1024 < t.m <= 4096
-    X = [t.instantiate(lmp[k], load[k] * 1e3) for k in range(N)]
-    b, c, u = (np.array([x[i] for x in X]) for i in (1, 0, 2))
-    kc = np.array([x[3] for x in X])
-    r = ID.solve_batch(t.A, b, c, u)
-    ref = np.array([H.solve(L.solar_battery_hydrogen_raw(lmp[k], True, PAR, pv_cfs=cfs, load_mw=load[k], reserve_mw=np.full(T, 100.0)))[0]
-                    for k in range(N)])
-    assert (r["status"] == ID.OPTIMAL).all(), r["status"]
-    assert (np.abs(r["obj"] + kc - ref) / np.abs(ref)).max() < 1e-8
-    tp = TP.solar_battery_hydrogen_design(T, None, **PAR)
-    cf2 = np.clip(cfs[None] * np.random.default_rng(T).uniform(0.5, 1.0, (N, T)), 0, 1)
-    rp = TP.solar_design_rparams(T, load, cf2, np.full((N, T), 100.0))
-    for k in range(N):
-        c, b, u, kk = tp.instantiate(lmp[k], rp[k])
-        rk = ID.solve_batch(tp.matrix(rp[k]), b[None], c[None], u[None], rho=tp.meta.get("reg_primal", 1e-8))
-        ref = H.solve(L.solar_battery_hydrogen_raw(lmp[k], True, PAR, pv_cfs=cf2[k], load_mw=load[k], reserve_mw=np.full(T, 100.0)))[0]
-        assert rk["status"][0] == ID.OPTIMAL
-        assert abs(rk["obj"][0] + kk - ref) / abs(ref) < 1e-8
+    LP, against the certified exact optima (real_lps, the sets the GPU suite runs the cluster kernel on) through check_exact, and
+    within 1e-8 of the exact objective.  The mirror at T = 168 (m = 2 523) is not run here: it takes about a minute per LP."""
+    procs = host_cores()
+    for pv, s in ((False, R.solar_design(T, 8, procs=procs)), (True, R.solar_design_pv(T, 8 if T == 72 else 6, procs=procs))):
+        assert 1024 < s.t.m <= 4096 and (s.t.amap is not None) == pv
+        q = s.take(np.array(MIRROR_LPS[pv]))
+        obj, status, x, y = [], [], [], []
+        for k in range(len(q)):
+            c, b, u, kk = q.t.instantiate(q.cparams[k], q.rparams[k])
+            r = ID.solve_batch(q.t.matrix(q.rparams[k]), b[None], c[None], u[None], rho=q.t.meta.get("reg_primal", 1e-8))
+            obj.append(r["obj"][0] + kk); status.append(r["status"][0]); x.append(r["x"][0]); y.append(r["y"][0])
+        assert (np.array(status) == ID.OPTIMAL).all(), status
+        e = R.check_exact(q, np.array(obj), np.array(status), np.stack(x), np.stack(y), what=(T, pv))
+        assert e["obj"] < 1e-8, e
+        print(T, "PV series per LP" if pv else "baked", R.fmt(e))
 
 
 def _desc(m, n, keep):

@@ -166,11 +166,10 @@ def test_design_lp_batches_against_highs(T, N):
     assert err.max() < 1e-6
 
 
-def test_status_rules():
-    """a negative bound is INFEASIBLE (NaN objective and rows, iters 0) with the neighbours untouched; max_iter = k reports 2k"""
+def _status_rules(kernel):
     pool = planted(65, 40, seed=5, N=4)
     t = pool.t
-    sol = S.BatchLPSolver(t, kernel=S.KERNEL_DENSE)
+    sol = S.BatchLPSolver(t, kernel=kernel)
     ref = sol.solve_host(pool.cparams, pool.rparams, want_x=True, want_y=True)
     rp = pool.rparams.copy()
     j = int(np.flatnonzero(np.isfinite(t.u0))[0])        # a bounded column: its bound comes from the umap terms
@@ -182,12 +181,23 @@ def test_status_rules():
     assert np.isnan(r.x[2]).all() and np.isnan(r.y[2]).all()
     keep = [0, 1, 3]
     assert np.array_equal(r.obj[keep], ref.obj[keep]) and np.array_equal(r.x[keep], ref.x[keep])
-    r = S.BatchLPSolver(t, kernel=S.KERNEL_DENSE, max_iter=3).solve_host(pool.cparams, pool.rparams)
+    assert np.array_equal(r.y[keep], ref.y[keep]) and np.array_equal(r.iters[keep], ref.iters[keep])
+    r = S.BatchLPSolver(t, kernel=kernel, max_iter=3).solve_host(pool.cparams, pool.rparams)
     assert (r.status != S.OPTIMAL).all() and (r.iters == 6).all(), (r.status, r.iters)
 
 
-def test_status_parity_with_the_band_kernel():
-    """the LPs of test_kernel_status_parity (negative and boundary bounds, NaN price, infeasible row): same status as the band kernel"""
+def test_status_rules():
+    """a negative bound is INFEASIBLE (NaN objective and rows, iters 0) with the neighbours untouched; max_iter = k reports 2k (both
+    attempts counted)"""
+    _status_rules(S.KERNEL_DENSE)
+
+
+def test_status_rules_cluster():
+    """the same rules on the dense cluster kernel"""
+    _status_rules(S.KERNEL_DENSE_CLUSTER)
+
+
+def _status_parity(kernel):
     from test_kernel_status_parity import BAD, _family
     for name in ("stage2_T24", "chain_report48"):
         t, cp, rp, kw, ib, icf = _family(name)
@@ -202,8 +212,18 @@ def test_status_parity_with_the_band_kernel():
             cases.append(("infeasible_row", cp, rpi))
         for what, c, r in cases:
             band = S.BatchLPSolver(t, kernel=S.KERNEL_BAND).solve_host(c, r)
-            dn = S.BatchLPSolver(t, kernel=S.KERNEL_DENSE).solve_host(c, r)
-            assert np.array_equal(dn.status, band.status), (name, what, dn.status, band.status)
+            dn = S.BatchLPSolver(t, kernel=kernel).solve_host(c, r)
+            assert np.array_equal(dn.status, band.status), (name, what, kernel, dn.status, band.status)
+
+
+def test_status_parity_with_the_band_kernel():
+    """the LPs of test_kernel_status_parity (negative and boundary bounds, NaN price, infeasible row): same status as the band kernel"""
+    _status_parity(S.KERNEL_DENSE)
+
+
+def test_status_parity_of_the_cluster_kernel_with_the_band_kernel():
+    """the same LPs on the dense cluster kernel: same status as the band kernel"""
+    _status_parity(S.KERNEL_DENSE_CLUSTER)
 
 
 def test_refusals():

@@ -11,6 +11,7 @@ import real_lps as R
 from dispatches_b200 import lp_template as LT
 from dispatches_b200 import templates as TP
 from exact_lp import NotCertified, exact_optimum, highs_basis, kkt_residuals
+from oracle.highs import host_cores
 from planted_stage import XY_REL, planted_chain, planted_wb
 from test_planted_stage import _harness, needs_gxx
 
@@ -104,12 +105,37 @@ def test_solar_sets_certify(name):
     """the PV + battery + hydrogen LPs certify only through the repair: HiGHS drops the 1.2e-16 entry of sin(pi) or leaves row slacks
     and basic columns 1e-14 .. 1e-11 outside their bounds in exact arithmetic.  They are degenerate in x and y."""
     s = SOLAR[name]()
-    assert len(s) == 8 and s.pivots.max() > 0 and s.pivots.max() <= X.MAX_PIVOTS
+    assert len(s) == 8 and s.pivots.max() > 0 and s.pivots.max() <= X.max_pivots(s.t.m)
     assert not s.unique_x.any() and not s.unique_y.any()
     e = R.check_exact(s, s.obj, np.zeros(len(s), np.int32), s.x, s.y, what=name)
     assert max(e["primal"], e["bound"]) < 1e-13              # x* rounded to binary64: holdups of 1e6 mol next to flows of 1e-2
     if name.startswith("solar_design") and "_pv" not in name:
         assert 0.0 < np.abs(s.t.A.data).min() < 1e-15                # the sin(pi) hour, as the kernels receive it
+
+
+# the repair's pivots, LP by LP, on the 96-hour design LPs (m = 1 443): the baked set needs up to 95, past the 64 that used to be the
+# limit for every LP.  The counts are pinned so that a change of the repair's rules shows.
+LONG_DESIGN = {"solar_design96": (lambda: R.solar_design(96, 8, procs=host_cores()), [95, 58, 77, 81, 65, 70, 73, 45]),
+               "solar_design_pv96": (lambda: R.solar_design_pv(96, 6, procs=host_cores()), [49, 0, 0, 0, 8, 4])}
+
+
+@pytest.mark.parametrize("name", sorted(LONG_DESIGN))
+def test_long_design_sets_certify(name):
+    """the 96-hour design LPs certify through the repair, within its limit, and the repaired basis given back through basis= verifies
+    as it is, to the same optimum bit for bit (the week-long LPs, about 70 s each on one core, certify in the GPU suite)"""
+    make, pivots = LONG_DESIGN[name]
+    s = make()
+    assert s.t.m == 1443 and s.pivots.tolist() == pivots and s.pivots.max() < X.max_pivots(s.t.m)
+    assert not s.unique_x.any() and not s.unique_y.any()
+    e = R.check_exact(s, s.obj, np.zeros(len(s), np.int32), s.x, s.y, what=name)
+    assert max(e["primal"], e["bound"]) < 1e-13
+    k = int(np.argmax(s.pivots))
+    f = exact_optimum(s.t, s.cparams[k], s.rparams[k], basis=(s.col[k], s.row_basic[k]))
+    assert f.pivots == 0
+    for a, g in ((f.x, s.x[k]), (f.y, s.y[k]), (f.r, s.r[k]), (f.fixed, s.fixed[k]), (f.inside, s.inside[k]),
+                 (f.basis[0], s.col[k]), (f.basis[1], s.row_basic[k])):
+        assert np.array_equal(a, g)
+    assert f.obj == s.obj[k]
 
 
 @pytest.mark.parametrize("T", [24, 48])
