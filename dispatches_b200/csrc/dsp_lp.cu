@@ -1118,22 +1118,33 @@ int g_last_grid = 0, g_last_block = 0, g_last_smem = 0, g_last_ppc = 0;
         }                                                                                     \
     } while (0)
 
-template <class T>
-int upload(const std::vector<T> &h, T **d) {
-    *d = nullptr;
-    size_t bytes = std::max<size_t>(h.size(), 1) * sizeof(T);
-    CK(cudaMalloc((void **)d, bytes));
-    if (!h.empty()) {
-        cudaError_t e_ = cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice);
-        if (e_ != cudaSuccess) { cudaFree(*d); *d = nullptr; g_err = std::string("cudaMemcpy: ") + cudaGetErrorString(e_); return DSP_E_CUDA; }
-    }
-    return 0;
+// CSC of an m-row CSR matrix by a stable counting sort (rows ascending within a column); from[p] is the CSR position of CSC entry p
+struct Csc {
+    std::vector<int> ptr, idx, from;
+    std::vector<double> val;
+};
+Csc csc_of(int m, int n, const std::vector<int> &A_ptr, const std::vector<int> &A_idx, const std::vector<double> &A_val) {
+    const int nnz = A_ptr[m];
+    Csc C;
+    C.ptr.assign(n + 1, 0); C.idx.resize(nnz); C.from.resize(nnz); C.val.resize(nnz);
+    for (int q = 0; q < nnz; ++q) C.ptr[A_idx[q] + 1]++;
+    for (int j = 0; j < n; ++j) C.ptr[j + 1] += C.ptr[j];
+    std::vector<int> fill(C.ptr.begin(), C.ptr.end() - 1);
+    for (int i = 0; i < m; ++i)
+        for (int q = A_ptr[i]; q < A_ptr[i + 1]; ++q) {
+            const int dst = fill[A_idx[q]]++;
+            C.idx[dst] = i; C.val[dst] = A_val[q]; C.from[dst] = q;
+        }
+    return C;
 }
 
 }  // namespace
 
+// Made by `new dsp_template()`: value-initialised, so every field not set at creation is zero.
 struct dsp_template {
     KParams kp;
+    enum Kind { BAND, DENSE, DENSE_CLUSTER } kind;   // DENSE (_CLUSTER): made by dsp_lp_template_create_dense (_cluster), no band
+                                                     // data, only the dense (cluster) kernel runs
     bool has_stage;
     mutable double *ws;            // global workspace for templates whose work region exceeds shared memory
     mutable size_t ws_bytes;
@@ -1148,8 +1159,13 @@ struct dsp_template {
     int smem_optin;
     size_t ws_cap;                 // largest global workspace a launch may allocate: a quarter of device memory
     std::vector<void *> dev_allocs;
-    std::vector<int> col_perm, row_perm;     // dsp_lp_template_create_csr: caller index of internal column / row
-    std::vector<int> csr_ptr, csr_idx, asm_qa, asm_qb;   // permuted CSR pattern + assembly factor positions (kept for matrix parameters)
+    std::vector<int> col_perm, row_perm;     // dsp_lp_template_create_csr / _dense: caller index of internal column / row
+    std::vector<int> asm_qa, asm_qb;         // dsp_lp_template_create_csr: the two CSR positions of every assembly term
+    struct Band {                  // a band template's matrix in internal order: exactly what its hot blob packs
+        std::vector<int> A_ptr, A_idx, asm_ptr, asm_col;    // CSR; band assembly list padded to half bandwidth kp.w
+        std::vector<double> A_val, asm_val;
+        Csc At;
+    } band;
     unsigned long long *ticket;
     // host-call staging (pinned) and device buffers, grown on demand
     int64_t cap_N;
@@ -1161,8 +1177,6 @@ struct dsp_template {
     int64_t cap_rp_rows;
     cudaStream_t stream, stream2;
     std::atomic<int> busy;         // a host call is in flight on this handle (staging buffers, streams and ticket are per handle)
-    bool dense_only;               // made by dsp_lp_template_create_dense: no band data, only the dense kernel runs
-    bool cluster_only;             // made by dsp_lp_template_create_dense_cluster: no band data, only the dense cluster kernel runs
     struct Dense {                 // the dense kernel's data (dense templates; band templates: built at the first DSP_KERNEL_DENSE call)
         bool ready;
         int nt, nent;
@@ -1247,6 +1261,25 @@ int allow_smem(F fn, size_t bytes) {
     return 0;
 }
 
+// copies cnt elements of src into a new device allocation owned by the handle (dsp_lp_template_destroy releases it, also after an error)
+template <class V>
+int upload(dsp_template *T, const V *src, size_t cnt, const V **dst) {
+    V *d = nullptr;
+    CK(cudaMalloc((void **)&d, std::max<size_t>(cnt, 1) * sizeof(V)));
+    T->dev_allocs.push_back(d);
+    if (cnt) CK(cudaMemcpy(d, src, cnt * sizeof(V), cudaMemcpyHostToDevice));
+    *dst = d;
+    return 0;
+}
+template <class V>
+int upload(dsp_template *T, const std::vector<V> &v, const V **dst) { return upload(T, v.data(), v.size(), dst); }
+
+// releases a handle under construction at every error return; t = nullptr hands it to the caller
+struct Guard {
+    dsp_template *t;
+    ~Guard() { if (t) dsp_lp_template_destroy(t); }
+};
+
 int check_maps(const dsp_template_desc *D) {
     for (int q = 0; q < D->cmap.ptr[D->n]; ++q)
         if (D->cmap.idx[q] < 0 || D->cmap.idx[q] >= D->Pc) { g_err = "cmap.idx out of range"; return DSP_E_ARG; }
@@ -1261,16 +1294,6 @@ int check_maps(const dsp_template_desc *D) {
 // parameter maps of c, b, u and the objective constant (D's matrix and assembly fields are not read)
 int template_init(dsp_template *T, const dsp_template_desc *D) {
     const int m = D->m, n = D->n, nb = D->nb;
-    memset(&T->kp, 0, sizeof(KParams));
-    T->cap_N = 0; T->cap_x = T->cap_y = false; T->cap_rp_rows = 0;
-    T->has_stage = false; T->has_chain1 = false; T->stage_blocks_per_sm = 0; T->ws = nullptr; T->ws_bytes = 0;
-    T->h_cp = T->h_rp = T->h_obj = T->h_x = T->h_y = nullptr; T->h_status = T->h_iters = nullptr;
-    T->d_cp = T->d_rp = T->d_obj = T->d_x = T->d_y = nullptr; T->d_status = T->d_iters = nullptr;
-    T->stream = nullptr; T->stream2 = nullptr; T->busy.store(0);
-    T->dense_only = false;
-    T->cluster_only = false;
-    memset(&T->dn, 0, sizeof(T->dn));
-    memset(&T->spl, 0, sizeof(T->spl));
     CK(cudaGetDevice(&T->device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, T->device));
@@ -1280,45 +1303,35 @@ int template_init(dsp_template *T, const dsp_template_desc *D) {
     KParams &K = T->kp;
     K.m = m; K.n = n; K.nb = nb; K.Pc = D->Pc; K.Pr = D->Pr;
     K.o0 = D->o0;
-    auto up_d = [&](const double *src, size_t cnt, const double **dst) -> int {
-        std::vector<double> v(src, src + cnt);
-        double *d;
-        int rc = upload(v, &d);
-        if (rc) return rc;
-        T->dev_allocs.push_back(d);
-        *dst = d;
-        return 0;
-    };
-    auto up_i = [&](const int32_t *src, size_t cnt, const int **dst) -> int {
-        std::vector<int> v(src, src + cnt);
-        int *d;
-        int rc = upload(v, &d);
-        if (rc) return rc;
-        T->dev_allocs.push_back(d);
-        *dst = d;
-        return 0;
-    };
-    int rc = 0;
-    rc |= up_d(D->c0, n, &K.c0);
-    rc |= up_d(D->b0, m, &K.b0);
-    rc |= up_d(D->u0, nb, &K.u0);
-    rc |= up_d(D->omap, D->Pr, &K.omap);
-    rc |= up_d(D->ocmap, D->Pc, &K.ocmap);
-    rc |= up_i(D->cmap.ptr, n + 1, &K.cm_ptr);
-    rc |= up_i(D->cmap.idx, D->cmap.ptr[n], &K.cm_idx);
-    rc |= up_d(D->cmap.val, D->cmap.ptr[n], &K.cm_val);
-    rc |= up_i(D->bmap.ptr, m + 1, &K.bm_ptr);
-    rc |= up_i(D->bmap.idx, D->bmap.ptr[m], &K.bm_idx);
-    rc |= up_d(D->bmap.val, D->bmap.ptr[m], &K.bm_val);
-    rc |= up_i(D->umap.ptr, nb + 1, &K.um_ptr);
-    rc |= up_i(D->umap.idx, D->umap.ptr[nb], &K.um_idx);
-    rc |= up_d(D->umap.val, D->umap.ptr[nb], &K.um_val);
-    if (rc) return DSP_E_CUDA;
+    if (upload(T, D->c0, n, &K.c0) || upload(T, D->b0, m, &K.b0) || upload(T, D->u0, nb, &K.u0) ||
+        upload(T, D->omap, D->Pr, &K.omap) || upload(T, D->ocmap, D->Pc, &K.ocmap) ||
+        upload(T, D->cmap.ptr, n + 1, &K.cm_ptr) || upload(T, D->cmap.idx, D->cmap.ptr[n], &K.cm_idx) ||
+        upload(T, D->cmap.val, D->cmap.ptr[n], &K.cm_val) ||
+        upload(T, D->bmap.ptr, m + 1, &K.bm_ptr) || upload(T, D->bmap.idx, D->bmap.ptr[m], &K.bm_idx) ||
+        upload(T, D->bmap.val, D->bmap.ptr[m], &K.bm_val) ||
+        upload(T, D->umap.ptr, nb + 1, &K.um_ptr) || upload(T, D->umap.idx, D->umap.ptr[nb], &K.um_idx) ||
+        upload(T, D->umap.val, D->umap.ptr[nb], &K.um_val))
+        return DSP_E_CUDA;
     CK(cudaMalloc((void **)&T->ticket, 16 * sizeof(unsigned long long)));
     T->dev_allocs.push_back(T->ticket);
     CK(cudaStreamCreateWithFlags(&T->stream, cudaStreamNonBlocking));
     CK(cudaStreamCreateWithFlags(&T->stream2, cudaStreamNonBlocking));
     return 0;
+}
+
+// the batch fields and dimensions every family's parameter struct shares with KParams by name
+template <class Q>
+void copy_batch(Q &q, const KParams &K) {
+    q.N = K.N; q.cparams = K.cparams; q.rparams = K.rparams; q.rstride = K.rstride; q.Pc = K.Pc; q.Pr = K.Pr;
+    q.omap = K.omap; q.ocmap = K.ocmap; q.o0 = K.o0;
+    q.tol = K.tol; q.feas_tol = K.feas_tol; q.step_frac = K.step_frac; q.reg = K.reg; q.max_iter = K.max_iter;
+    q.obj = K.obj; q.x_out = K.x_out; q.y_out = K.y_out; q.status = K.status; q.iters = K.iters; q.n = K.n; q.m = K.m; q.ticket = K.ticket;
+}
+// the parameter maps c = c0 + Cmap cp, b = b0 + Bmap rp, u = u0 + Umap rp over the first nb columns
+template <class Q>
+void copy_maps(Q &q, const KParams &K) {
+    q.nb = K.nb; q.c0 = K.c0; q.b0 = K.b0; q.u0 = K.u0; q.cm_ptr = K.cm_ptr; q.cm_idx = K.cm_idx; q.cm_val = K.cm_val;
+    q.bm_ptr = K.bm_ptr; q.bm_idx = K.bm_idx; q.bm_val = K.bm_val; q.um_ptr = K.um_ptr; q.um_idx = K.um_idx; q.um_val = K.um_val;
 }
 
 // per-problem matrix terms of a dense template, in the caller's order: CSR position (internal order), rparams index, coefficient
@@ -1335,31 +1348,20 @@ struct DenseTerms {
 constexpr long long kDenseMaxTerms = 1LL << 26;
 int dense_build(dsp_template *T, const std::vector<int> &A_ptr, const std::vector<int> &A_idx, const std::vector<double> &A_val,
                 const DenseTerms *terms = nullptr) {
-    const int m = T->kp.m, n = T->kp.n, nnz = A_ptr[m];
+    const int m = T->kp.m, n = T->kp.n;
     const int TS = dense::TS;
     const bool per_lp = terms && !terms->q.empty();
-    std::vector<int> At_ptr(n + 1, 0), At_idx(nnz), at_from(nnz);
-    std::vector<double> At_val(nnz);
-    for (int q = 0; q < nnz; ++q) At_ptr[A_idx[q] + 1]++;
-    for (int j = 0; j < n; ++j) At_ptr[j + 1] += At_ptr[j];
-    {
-        std::vector<int> fill(At_ptr.begin(), At_ptr.end() - 1);
-        for (int i = 0; i < m; ++i)
-            for (int q = A_ptr[i]; q < A_ptr[i + 1]; ++q) {
-                const int dst = fill[A_idx[q]]++;
-                At_idx[dst] = i; At_val[dst] = A_val[q]; at_from[dst] = q;
-            }
-    }
+    const Csc At = csc_of(m, n, A_ptr, A_idx, A_val);
     long long nterms = 0;
-    for (int j = 0; j < n; ++j) { const long long c = At_ptr[j + 1] - At_ptr[j]; nterms += c * (c + 1) / 2; }
+    for (int j = 0; j < n; ++j) { const long long c = At.ptr[j + 1] - At.ptr[j]; nterms += c * (c + 1) / 2; }
     if (nterms > kDenseMaxTerms) { g_err = "dense kernel: the assembly list of A A' has more than 2^26 products"; return DSP_E_ARG; }
     // entries of the lower pattern (a >= b), first seen order; then sorted by workspace position
     std::vector<int> slot((size_t)m * m, -1), cnt;
     std::vector<long long> pos;
     for (int j = 0; j < n; ++j)
-        for (int qa = At_ptr[j]; qa < At_ptr[j + 1]; ++qa)
-            for (int qb = At_ptr[j]; qb <= qa; ++qb) {
-                const int a = At_idx[qa], b = At_idx[qb];      // rows ascending within a column: a >= b
+        for (int qa = At.ptr[j]; qa < At.ptr[j + 1]; ++qa)
+            for (int qb = At.ptr[j]; qb <= qa; ++qb) {
+                const int a = At.idx[qa], b = At.idx[qb];      // rows ascending within a column: a >= b
                 int &e = slot[(size_t)a * m + b];
                 if (e < 0) {
                     e = (int)pos.size();
@@ -1379,29 +1381,19 @@ int dense_build(dsp_template *T, const std::vector<int> &A_ptr, const std::vecto
     for (int r = 0; r < nent; ++r) { asm_pos[r] = (int)pos[order[r]]; asm_ptr[r + 1] = asm_ptr[r] + cnt[order[r]]; }
     std::vector<int> fill(asm_ptr.begin(), asm_ptr.end() - 1);
     for (int j = 0; j < n; ++j)
-        for (int qa = At_ptr[j]; qa < At_ptr[j + 1]; ++qa)
-            for (int qb = At_ptr[j]; qb <= qa; ++qb) {
-                const int r = rank[slot[(size_t)At_idx[qa] * m + At_idx[qb]]];
+        for (int qa = At.ptr[j]; qa < At.ptr[j + 1]; ++qa)
+            for (int qb = At.ptr[j]; qb <= qa; ++qb) {
+                const int r = rank[slot[(size_t)At.idx[qa] * m + At.idx[qb]]];
                 asm_col[fill[r]] = j;
-                if (per_lp) { asm_qa[fill[r]] = at_from[qa]; asm_qb[fill[r]] = at_from[qb]; }
-                asm_val[fill[r]++] = At_val[qa] * At_val[qb];
+                if (per_lp) { asm_qa[fill[r]] = At.from[qa]; asm_qb[fill[r]] = At.from[qb]; }
+                asm_val[fill[r]++] = At.val[qa] * At.val[qb];
             }
     dsp_template::Dense &D = T->dn;
-    int *pi; double *pd;
-    auto ui = [&](const std::vector<int> &v, const int **dst) { int rc = upload(v, &pi); if (!rc) { T->dev_allocs.push_back(pi); *dst = pi; } return rc; };
-    auto ud = [&](const std::vector<double> &v, const double **dst) { int rc = upload(v, &pd); if (!rc) { T->dev_allocs.push_back(pd); *dst = pd; } return rc; };
-    int rc = 0;
-    rc = rc ? rc : ui(A_ptr, &D.A_ptr);
-    rc = rc ? rc : ui(A_idx, &D.A_idx);
-    rc = rc ? rc : ud(A_val, &D.A_val);
-    rc = rc ? rc : ui(At_ptr, &D.At_ptr);
-    rc = rc ? rc : ui(At_idx, &D.At_idx);
-    rc = rc ? rc : ud(At_val, &D.At_val);
-    rc = rc ? rc : ui(asm_pos, &D.asm_pos);
-    rc = rc ? rc : ui(asm_ptr, &D.asm_ptr);
-    rc = rc ? rc : ui(asm_col, &D.asm_col);
-    rc = rc ? rc : ud(asm_val, &D.asm_val);
-    if (rc) return rc;
+    if (upload(T, A_ptr, &D.A_ptr) || upload(T, A_idx, &D.A_idx) || upload(T, A_val, &D.A_val) ||
+        upload(T, At.ptr, &D.At_ptr) || upload(T, At.idx, &D.At_idx) || upload(T, At.val, &D.At_val) ||
+        upload(T, asm_pos, &D.asm_pos) || upload(T, asm_ptr, &D.asm_ptr) || upload(T, asm_col, &D.asm_col) ||
+        upload(T, asm_val, &D.asm_val))
+        return DSP_E_CUDA;
     CK(cudaFuncSetAttribute(dsp_ipm_dense_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
     if (per_lp) {
         // the terms grouped by CSR position, each group in the caller's order (the order the band kernel adds them in)
@@ -1416,14 +1408,10 @@ int dense_build(dsp_template *T, const std::vector<int> &A_ptr, const std::vecto
             am_ptr.back()++;
             am_param[k] = terms->param[by[k]]; am_coef[k] = terms->coef[by[k]];
         }
-        rc = rc ? rc : ui(am_q, &D.am_q);
-        rc = rc ? rc : ui(am_ptr, &D.am_ptr);
-        rc = rc ? rc : ui(am_param, &D.am_param);
-        rc = rc ? rc : ud(am_coef, &D.am_coef);
-        rc = rc ? rc : ui(at_from, &D.at_from);
-        rc = rc ? rc : ui(asm_qa, &D.asm_qa);
-        rc = rc ? rc : ui(asm_qb, &D.asm_qb);
-        if (rc) return rc;
+        if (upload(T, am_q, &D.am_q) || upload(T, am_ptr, &D.am_ptr) || upload(T, am_param, &D.am_param) ||
+            upload(T, am_coef, &D.am_coef) || upload(T, At.from, &D.at_from) || upload(T, asm_qa, &D.asm_qa) ||
+            upload(T, asm_qb, &D.asm_qb))
+            return DSP_E_CUDA;
         CK(cudaFuncSetAttribute(dsp_ipm_dense_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
         D.n_amq = (int)am_q.size();
         D.nterms = nterms;
@@ -1498,78 +1486,50 @@ int dsp_lp_template_create(const dsp_template_desc *D, dsp_template **out) {
         g_err = "dsp_lp_template_create: bad dimensions";
         return DSP_E_ARG;
     }
-    const int m = D->m, n = D->n, nb = D->nb, w = D->w;
+    const int m = D->m, n = D->n, w = D->w;
     const int nnz = D->A_ptr[m];
     // the kernels are instantiated for half bandwidths 1, 2, 4, 8, 16, 32: pad the band storage to the next one
     int wt = 1;
     while (wt < w) wt *= 2;
     if (wt > 32) { g_err = "dsp_lp_template_create: half bandwidth of A*A' above 32 is not supported"; return DSP_E_ARG; }
-    const int nent = m * (wt + 1);
     const int nasm = D->asm_ptr[m * (w + 1)];
-    std::vector<int> asm_ptr_pad(nent + 1, 0);
-    for (int i = 0; i < m; ++i)
-        for (int k = 0; k <= wt; ++k) {
-            const int cnt = (k <= w) ? D->asm_ptr[i * (w + 1) + k + 1] - D->asm_ptr[i * (w + 1) + k] : 0;
-            asm_ptr_pad[i * (wt + 1) + k + 1] = asm_ptr_pad[i * (wt + 1) + k] + cnt;
-        }
     for (int q = 0; q < nasm; ++q)
         if (D->asm_col[q] < 0 || D->asm_col[q] >= n) { g_err = "asm_col out of range"; return DSP_E_ARG; }
     if (int rc = check_maps(D)) return rc;
-    // CSC of A
-    std::vector<int> At_ptr(n + 1, 0), At_idx(nnz);
-    std::vector<double> At_val(nnz);
-    for (int q = 0; q < nnz; ++q) {
+    for (int q = 0; q < nnz; ++q)
         if (D->A_idx[q] < 0 || D->A_idx[q] >= n) { g_err = "A_idx out of range"; return DSP_E_ARG; }
-        At_ptr[D->A_idx[q] + 1]++;
-    }
-    for (int j = 0; j < n; ++j) At_ptr[j + 1] += At_ptr[j];
-    {
-        std::vector<int> fill(At_ptr.begin(), At_ptr.end() - 1);
-        for (int i = 0; i < m; ++i)
-            for (int q = D->A_ptr[i]; q < D->A_ptr[i + 1]; ++q) {
-                int dst = fill[D->A_idx[q]]++;
-                At_idx[dst] = i;
-                At_val[dst] = D->A_val[q];
-            }
-    }
-    // hot blob
-    size_t dbl = (size_t)nnz * 2 + nasm;
-    size_t ints = (size_t)(m + 1) + nnz + (n + 1) + nnz + (nent + 1) + nasm;
-    size_t hot_bytes = dbl * 8 + ints * 4;
-    hot_bytes = (hot_bytes + 15) / 16 * 16;
-    std::vector<unsigned char> hot(hot_bytes, 0);
-    {
-        double *pd = (double *)hot.data();
-        memcpy(pd, D->A_val, (size_t)nnz * 8); pd += nnz;
-        memcpy(pd, At_val.data(), (size_t)nnz * 8); pd += nnz;
-        memcpy(pd, D->asm_val, (size_t)nasm * 8); pd += nasm;
-        int *pi = (int *)pd;
-        memcpy(pi, D->A_ptr, (size_t)(m + 1) * 4); pi += m + 1;
-        memcpy(pi, D->A_idx, (size_t)nnz * 4); pi += nnz;
-        memcpy(pi, At_ptr.data(), (size_t)(n + 1) * 4); pi += n + 1;
-        memcpy(pi, At_idx.data(), (size_t)nnz * 4); pi += nnz;
-        memcpy(pi, asm_ptr_pad.data(), (size_t)(nent + 1) * 4); pi += nent + 1;
-        memcpy(pi, D->asm_col, (size_t)nasm * 4);
-    }
     dsp_template *T = new dsp_template();
-    struct Guard {      // every error return below releases the handle and its device allocations
-        dsp_template *t;
-        ~Guard() { if (t) dsp_lp_template_destroy(t); }
-    } guard{T};
+    Guard guard{T};
+    dsp_template::Band &B = T->band;
+    B.A_ptr.assign(D->A_ptr, D->A_ptr + m + 1);
+    B.A_idx.assign(D->A_idx, D->A_idx + nnz);
+    B.A_val.assign(D->A_val, D->A_val + nnz);
+    B.At = csc_of(m, n, B.A_ptr, B.A_idx, B.A_val);
+    B.asm_ptr.assign((size_t)m * (wt + 1) + 1, 0);
+    for (int i = 0; i < m; ++i)
+        for (int k = 0; k <= wt; ++k) {
+            const int cnt = (k <= w) ? D->asm_ptr[i * (w + 1) + k + 1] - D->asm_ptr[i * (w + 1) + k] : 0;
+            B.asm_ptr[i * (wt + 1) + k + 1] = B.asm_ptr[i * (wt + 1) + k] + cnt;
+        }
+    B.asm_col.assign(D->asm_col, D->asm_col + nasm);
+    B.asm_val.assign(D->asm_val, D->asm_val + nasm);
+    // hot blob, in the order hot_views reads it: the values of A, A' and the assembly list, then the index arrays; 16-byte padded
+    std::vector<unsigned char> hot;
+    auto pack = [&hot](const auto &v) {
+        const size_t at = hot.size(), bytes = v.size() * sizeof(v[0]);
+        hot.resize(at + bytes);
+        if (bytes) memcpy(hot.data() + at, v.data(), bytes);
+    };
+    pack(B.A_val); pack(B.At.val); pack(B.asm_val);
+    pack(B.A_ptr); pack(B.A_idx); pack(B.At.ptr); pack(B.At.idx); pack(B.asm_ptr); pack(B.asm_col);
+    hot.resize((hot.size() + 15) / 16 * 16, 0);
     if (int rc = template_init(T, D)) return rc;
     KParams &K = T->kp;
     K.w = wt; K.nnz = nnz; K.nasm = nasm;
-    K.hot_bytes = (int)hot_bytes;
-    {
-        unsigned char *d;
-        int rc = upload(hot, &d);
-        if (rc) return rc;
-        T->dev_allocs.push_back(d);
-        K.hot_g = d;
-    }
+    K.hot_bytes = (int)hot.size();
+    if (int rc = upload(T, hot, &K.hot_g)) return rc;
     K.band_doubles = (m + 2 * wt) + (m + 2 * wt) * (wt + 1);
-    K.prob_doubles = 8 * n + 6 * nb + 3 * m + K.band_doubles;
-    K.hybrid = 0;
+    K.prob_doubles = 8 * n + 6 * D->nb + 3 * m + K.band_doubles;
     for (int bw = 1; bw <= 32; bw *= 2)
         for (int placement = 0; placement < 3; ++placement)       // workspace, shared memory + staged template, shared memory
             CK(cudaFuncSetAttribute(band_kernel(bw, placement == 0, placement == 1), cudaFuncAttributeMaxDynamicSharedMemorySize, T->smem_optin));
@@ -1590,18 +1550,13 @@ int dsp_lp_template_set_stage_wb(dsp_template *T, const dsp_stage_wb_desc *d) {
     std::vector<int> ci(d->col_idx, d->col_idx + 7 * d->T), ri(d->row_idx, d->row_idx + 4 * d->T);
     for (int v : ci) if (v < -1 || v >= T->kp.n) { g_err = "col_idx out of range"; return DSP_E_ARG; }
     for (int v : ri) if (v < 0 || v >= T->kp.m) { g_err = "row_idx out of range"; return DSP_E_ARG; }
-    int *dci, *dri;
-    int rc = upload(ci, &dci); if (rc) return rc;
-    rc = upload(ri, &dri); if (rc) return rc;
-    T->dev_allocs.push_back(dci); T->dev_allocs.push_back(dri);
-    S.col_idx = dci; S.row_idx = dri;
+    if (upload(T, ci, &S.col_idx) || upload(T, ri, &S.row_idx)) return DSP_E_CUDA;
     int nb = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, dsp_ipm_stage_wb_kernel, 32 * kStageWarps, 0));
     T->stage_blocks_per_sm = std::max(nb, 1);
     if (d->T <= kStage2MaxT) {
         const Stage2Geom g = stage2_geometry(d->T);
-        rc = allow_smem(stage2_kernel(g), stage2_smem_bytes(g) * kStage2Warps);
-        if (rc) return rc;
+        if (int rc = allow_smem(stage2_kernel(g), stage2_smem_bytes(g) * kStage2Warps)) return rc;
     }
     T->has_stage = true;
     return 0;
@@ -1628,16 +1583,11 @@ int dsp_lp_template_set_stage_chain1(dsp_template *T, const dsp_stage_chain1_des
     for (int k = 0; k < T->kp.m; ++k) rpos[T->row_perm.empty() ? k : T->row_perm[k]] = k;
     for (int &v : ci) if (v >= 0) v = cpos[v];
     for (int &v : ri) v = rpos[v];
-    std::vector<double> cf(d->coef, d->coef + (size_t)d->T * NC), cn(d->coef_next, d->coef_next + d->T);
-    int *dci, *dri; double *dcf, *dcn;
-    int rc = upload(ci, &dci); if (rc) return rc; T->dev_allocs.push_back(dci);
-    rc = upload(ri, &dri); if (rc) return rc; T->dev_allocs.push_back(dri);
-    rc = upload(cf, &dcf); if (rc) return rc; T->dev_allocs.push_back(dcf);
-    rc = upload(cn, &dcn); if (rc) return rc; T->dev_allocs.push_back(dcn);
+    if (upload(T, ci, &T->c1_col_idx) || upload(T, ri, &T->c1_row_idx) || upload(T, d->coef, (size_t)d->T * NC, &T->c1_coef) ||
+        upload(T, d->coef_next, (size_t)d->T, &T->c1_coef_next))
+        return DSP_E_CUDA;
     T->c1_T = d->T; T->c1_NF = d->NF;
-    T->c1_col_idx = dci; T->c1_row_idx = dri; T->c1_coef = dcf; T->c1_coef_next = dcn;
-    rc = allow_smem(chain1_kernel(chain1_lanes(d->T), d->NF), chain1_smem_bytes(d->NF) * chain1_warps(d->NF));
-    if (rc) return rc;
+    if (int rc = allow_smem(chain1_kernel(chain1_lanes(d->T), d->NF), chain1_smem_bytes(d->NF) * chain1_warps(d->NF))) return rc;
     T->has_chain1 = true;
     return 0;
 }
@@ -1694,6 +1644,34 @@ BandGeom band_geometry(const dsp_template *T, const KParams &K) {
     return g;
 }
 
+// The kernel family a batch runs, chosen by kernel_family from the template and dsp_opts::kernel
+enum Family { F_BAND, F_BAND_SPLIT, F_STAGE2, F_STAGE2_LONG, F_STAGE_V1, F_CHAIN1, F_DENSE, F_DENSE_CLUSTER };
+
+// A dense (cluster) template runs only its own kernel; DSP_KERNEL_AUTO takes a registered stage kernel, else the band kernel; an
+// unknown kernel value runs the band kernel.
+static int kernel_family(const dsp_template *T, int k, Family *f) {
+    if (T->kind == dsp_template::DENSE_CLUSTER && k != DSP_KERNEL_AUTO && k != DSP_KERNEL_DENSE_CLUSTER) {
+        g_err = "dsp_lp_solve_batch: a template made by dsp_lp_template_create_dense_cluster runs only the dense cluster kernel (DSP_KERNEL_AUTO or DSP_KERNEL_DENSE_CLUSTER)";
+        return DSP_E_ARG;
+    }
+    if (T->kind == dsp_template::DENSE && k != DSP_KERNEL_AUTO && k != DSP_KERNEL_DENSE) {
+        g_err = "dsp_lp_solve_batch: a template made by dsp_lp_template_create_dense runs only the dense kernel (DSP_KERNEL_AUTO or DSP_KERNEL_DENSE)";
+        return DSP_E_ARG;
+    }
+    const bool stage = k == DSP_KERNEL_AUTO || k == DSP_KERNEL_STAGE;
+    if (T->kind == dsp_template::DENSE_CLUSTER || k == DSP_KERNEL_DENSE_CLUSTER) *f = F_DENSE_CLUSTER;
+    else if (T->kind == dsp_template::DENSE || k == DSP_KERNEL_DENSE) *f = F_DENSE;
+    else if (k == DSP_KERNEL_BAND_SPLIT) *f = F_BAND_SPLIT;
+    else if (T->has_stage && stage) *f = T->sp.T > kStage2MaxT ? F_STAGE2_LONG : F_STAGE2;
+    else if (T->has_stage && k == DSP_KERNEL_STAGE_V1) *f = F_STAGE_V1;
+    else if (T->has_chain1 && stage) *f = F_CHAIN1;
+    else if (k == DSP_KERNEL_STAGE || k == DSP_KERNEL_STAGE_V1) {
+        g_err = "dsp_lp_solve_batch: the template has no stage descriptor";
+        return DSP_E_ARG;
+    } else *f = F_BAND;
+    return 0;
+}
+
 // grows the handle's global workspace to at least `need` bytes, once the kernels already queued on the stream are done with it
 static int grow_ws(const dsp_template *T, size_t need, cudaStream_t st) {
     if (need <= T->ws_bytes) return 0;
@@ -1703,6 +1681,18 @@ static int grow_ws(const dsp_template *T, size_t need, cudaStream_t st) {
     CK(cudaMalloc((void **)&T->ws, need));
     T->ws_bytes = need;
     return 0;
+}
+
+// A persistent grid whose units (warps, CTAs or clusters: one LP each in flight) have regions of unit_bytes in the handle's workspace:
+// as many units as are co-resident (`resident`) and as the batch has, halved until their regions fit under the workspace cap; up to
+// max_per_block units per block, spread one per block while there are fewer than SMs x max_per_block.  Grows the workspace to fit.
+struct WsGrid { long long blocks; int per_block; };
+static int ws_grid(const dsp_template *T, long long N, long long resident, int max_per_block, size_t unit_bytes, cudaStream_t st, WsGrid *g) {
+    long long units = std::min<long long>(N, resident);
+    while (units > 1 && (size_t)units * unit_bytes > T->ws_cap) units /= 2;
+    g->per_block = (int)std::min<long long>(max_per_block, std::max<long long>(1, units / T->sm_count));
+    g->blocks = (units + g->per_block - 1) / g->per_block;
+    return grow_ws(T, (size_t)g->blocks * g->per_block * unit_bytes, st);
 }
 
 // checks the launch just issued and records its geometry for dsp_lp_launch_count / dsp_lp_last_launch
@@ -1717,10 +1707,7 @@ static int launched(long long grid, long long block, size_t smem, long long ppc)
 // parameters of the stage-2 kernels (short and long horizon): the batch in K, the stage structure of the template
 static stage2::Params stage2_params(const dsp_template *T, const KParams &K) {
     stage2::Params Q;
-    Q.N = K.N; Q.cparams = K.cparams; Q.rparams = K.rparams; Q.rstride = K.rstride; Q.Pc = K.Pc; Q.Pr = K.Pr;
-    Q.omap = K.omap; Q.ocmap = K.ocmap; Q.o0 = K.o0;
-    Q.tol = K.tol; Q.feas_tol = K.feas_tol; Q.step_frac = K.step_frac; Q.reg = K.reg; Q.max_iter = K.max_iter;
-    Q.obj = K.obj; Q.x_out = K.x_out; Q.y_out = K.y_out; Q.status = K.status; Q.iters = K.iters; Q.n = K.n; Q.m = K.m; Q.ticket = K.ticket;
+    copy_batch(Q, K);
     const stagewb::StageParams &S = T->sp;
     Q.T = S.T; Q.a = S.a; Q.binv = S.binv; Q.hf = S.hf; Q.dl = S.dl; Q.dur = S.dur; Q.krev = S.krev;
     Q.wcf_off = S.wcf_off; Q.p_off = S.p_off; Q.col_idx = S.col_idx; Q.row_idx = S.row_idx;
@@ -1731,22 +1718,18 @@ static stage2::Params stage2_params(const dsp_template *T, const KParams &K) {
 // long horizon (T > 96): one warp per LP, everything in a global workspace owned by the handle
 static int launch_stage2_long(const dsp_template *T, const KParams &K, cudaStream_t st) {
     const int P = (T->sp.T + 31) / 32;
-    const size_t per_warp = (size_t)stage2long::NW * P * 32 * sizeof(double);
     int occ = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dsp_ipm_stage2_long_kernel, 32 * kLongWarps, 0));
-    long long warps = std::min<long long>(K.N, (long long)T->sm_count * std::max(occ, 1) * kLongWarps);
-    while (warps > 1 && (size_t)warps * per_warp > T->ws_cap) warps /= 2;
-    // spread the warps over the SMs: one warp per CTA while there are fewer LPs than SMs x kLongWarps
-    const int wpb = (int)std::min<long long>(kLongWarps, std::max<long long>(1, warps / T->sm_count));
-    const long long blocks = (warps + wpb - 1) / wpb;
-    const int rc = grow_ws(T, (size_t)blocks * wpb * per_warp, st);
+    WsGrid g;
+    const int rc = ws_grid(T, K.N, (long long)T->sm_count * std::max(occ, 1) * kLongWarps, kLongWarps,
+                           (size_t)stage2long::NW * P * 32 * sizeof(double), st, &g);
     if (rc) return rc;
     stage2long::LongParams LQ;
     LQ.q = stage2_params(T, K);
     LQ.ws = T->ws; LQ.P = P;
     CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
-    dsp_ipm_stage2_long_kernel<<<(unsigned)blocks, 32 * wpb, 0, st>>>(LQ);
-    return launched(blocks, 32 * wpb, 0, wpb);
+    dsp_ipm_stage2_long_kernel<<<(unsigned)g.blocks, 32 * g.per_block, 0, st>>>(LQ);
+    return launched(g.blocks, 32 * g.per_block, 0, g.per_block);
 }
 
 // generation-2 stage kernel: 32/L LPs per warp, persistent CTAs, LP groups refill from the ticket counter
@@ -1792,12 +1775,8 @@ static int launch_chain1(const dsp_template *T, const KParams &K, cudaStream_t s
     const int wpb = (int)std::min<long long>(chain1_warps(NF), (warps_needed + blocks - 1) / blocks);
     const size_t smem = chain1_smem_bytes(NF) * wpb;
     chain1::Params Q;
-    Q.N = K.N; Q.cparams = K.cparams; Q.rparams = K.rparams; Q.rstride = K.rstride; Q.Pc = K.Pc; Q.Pr = K.Pr;
-    Q.omap = K.omap; Q.ocmap = K.ocmap; Q.o0 = K.o0;
-    Q.tol = K.tol; Q.feas_tol = K.feas_tol; Q.step_frac = K.step_frac; Q.reg = K.reg; Q.max_iter = K.max_iter;
-    Q.obj = K.obj; Q.x_out = K.x_out; Q.y_out = K.y_out; Q.status = K.status; Q.iters = K.iters; Q.n = K.n; Q.m = K.m; Q.nb = K.nb; Q.ticket = K.ticket;
-    Q.c0 = K.c0; Q.b0 = K.b0; Q.u0 = K.u0; Q.cm_ptr = K.cm_ptr; Q.cm_idx = K.cm_idx; Q.cm_val = K.cm_val;
-    Q.bm_ptr = K.bm_ptr; Q.bm_idx = K.bm_idx; Q.bm_val = K.bm_val; Q.um_ptr = K.um_ptr; Q.um_idx = K.um_idx; Q.um_val = K.um_val;
+    copy_batch(Q, K);
+    copy_maps(Q, K);
     Q.T = T->c1_T; Q.col_idx = T->c1_col_idx; Q.row_idx = T->c1_row_idx; Q.coef = T->c1_coef; Q.coef_next = T->c1_coef_next;
     Q.x_perm = K.xperm; Q.y_perm = K.yperm;
     CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
@@ -1832,14 +1811,14 @@ static int launch_band(const dsp_template *T, KParams K, cudaStream_t st) {
     return launched(ctas, warps * 32, smem, warps);
 }
 
-// the split band kernel's data of a band template (dsp_band_split.cuh), built from its device copy of A and of the band assembly list
+// the split band kernel's data of a band template (dsp_band_split.cuh), built from its host copy of A and of the band assembly list
 // at the first DSP_KERNEL_BAND_SPLIT call: rows cut into 32 chunks, a column on the lane of the first row it appears in, the CSR, CSC
 // and assembly list renumbered to split rows / columns
 static int ensure_split(const dsp_template *T) {
     static std::mutex mu;
     std::lock_guard<std::mutex> lk(mu);
     const KParams &K = T->kp;
-    const int W = K.w, m = K.m, n = K.n, nnz = K.nnz, nasm = K.nasm;
+    const int W = K.w, m = K.m, n = K.n;
     if (K.n_amap > 0) {
         g_err = "dsp_lp_solve_batch: DSP_KERNEL_BAND_SPLIT does not take per-problem matrix coefficients (dsp_lp_template_set_matrix_params); "
                 "use DSP_KERNEL_BAND";
@@ -1855,12 +1834,7 @@ static int ensure_split(const dsp_template *T) {
         return DSP_E_ARG;
     }
     if (T->spl.ready) return 0;
-    std::vector<unsigned char> hot(K.hot_bytes);
-    CK(cudaMemcpy(hot.data(), K.hot_g, hot.size(), cudaMemcpyDeviceToHost));
-    const double *A_val = (const double *)hot.data(), *asm_val = A_val + 2 * (size_t)nnz;
-    const int *A_ptr = (const int *)(asm_val + nasm), *A_idx = A_ptr + m + 1, *At_ptr = A_idx + nnz, *At_idx = At_ptr + n + 1;
-    const int *asm_ptr = At_idx + nnz, *asm_col = asm_ptr + m * (W + 1) + 1;
-    const double *At_val = A_val + nnz;
+    const dsp_template::Band &B = T->band;
     const int base = m / 32, rem = m % 32, Sr = base + (rem > 0);
     auto r0 = [&](int L) { return L * base + std::min(L, rem); };
     std::vector<int> rlane(m), rsplit(m);
@@ -1868,8 +1842,8 @@ static int ensure_split(const dsp_template *T) {
         for (int r = r0(L); r < r0(L + 1); ++r) { rlane[r] = L; rsplit[r] = (r - r0(L)) * 32 + L; }
     std::vector<int> owner(n, -1);
     for (int r = 0; r < m; ++r)
-        for (int q = A_ptr[r]; q < A_ptr[r + 1]; ++q)
-            if (owner[A_idx[q]] < 0) owner[A_idx[q]] = rlane[r];
+        for (int q = B.A_ptr[r]; q < B.A_ptr[r + 1]; ++q)
+            if (owner[B.A_idx[q]] < 0) owner[B.A_idx[q]] = rlane[r];
     std::vector<int> ccnt(32, 0), csplit(n);
     for (int c = 0; c < n; ++c) {
         const int L = std::max(owner[c], 0);       // a column in no row: lane 0
@@ -1884,52 +1858,31 @@ static int ensure_split(const dsp_template *T) {
     for (int r = 0; r < m; ++r) rnat[rsplit[r]] = r;
     for (size_t i = 0; i < rnat.size(); ++i) {
         if (const int r = rnat[i]; r >= 0)
-            for (int q = A_ptr[r]; q < A_ptr[r + 1]; ++q) { sA_idx.push_back(csplit[A_idx[q]]); sA_val.push_back(A_val[q]); }
+            for (int q = B.A_ptr[r]; q < B.A_ptr[r + 1]; ++q) { sA_idx.push_back(csplit[B.A_idx[q]]); sA_val.push_back(B.A_val[q]); }
         sA_ptr[i + 1] = (int)sA_idx.size();
     }
     for (size_t j = 0; j < cnat.size(); ++j) {
         if (const int c = cnat[j]; c >= 0)
-            for (int q = At_ptr[c]; q < At_ptr[c + 1]; ++q) { sAt_idx.push_back(rsplit[At_idx[q]]); sAt_val.push_back(At_val[q]); }
+            for (int q = B.At.ptr[c]; q < B.At.ptr[c + 1]; ++q) { sAt_idx.push_back(rsplit[B.At.idx[q]]); sAt_val.push_back(B.At.val[q]); }
         sAt_ptr[j + 1] = (int)sAt_idx.size();
     }
     for (int k = 0; k <= W; ++k)
         for (size_t i = 0; i < rnat.size(); ++i) {
             const size_t e = (size_t)k * Sr * 32 + i;
             if (const int r = rnat[i]; r >= 0)
-                for (int q = asm_ptr[r * (W + 1) + k]; q < asm_ptr[r * (W + 1) + k + 1]; ++q) {
-                    sasm_col.push_back(csplit[asm_col[q]]);
-                    sasm_val.push_back(asm_val[q]);
+                for (int q = B.asm_ptr[r * (W + 1) + k]; q < B.asm_ptr[r * (W + 1) + k + 1]; ++q) {
+                    sasm_col.push_back(csplit[B.asm_col[q]]);
+                    sasm_val.push_back(B.asm_val[q]);
                 }
             sasm_ptr[e + 1] = (int)sasm_col.size();
         }
     dsp_template *Tm = const_cast<dsp_template *>(T);
     dsp_template::Split &D = Tm->spl;
-    auto up_i = [&](const std::vector<int> &v, const int **dst) -> int {
-        int *d;
-        if (int rc = upload(v, &d)) return rc;
-        Tm->dev_allocs.push_back(d);
-        *dst = d;
-        return 0;
-    };
-    auto up_d = [&](const std::vector<double> &v, const double **dst) -> int {
-        double *d;
-        if (int rc = upload(v, &d)) return rc;
-        Tm->dev_allocs.push_back(d);
-        *dst = d;
-        return 0;
-    };
-    int rc = up_i(ccnt, &D.ccnt);
-    if (!rc) rc = up_i(cnat, &D.cnat);
-    if (!rc) rc = up_i(sA_ptr, &D.A_ptr);
-    if (!rc) rc = up_i(sA_idx, &D.A_idx);
-    if (!rc) rc = up_d(sA_val, &D.A_val);
-    if (!rc) rc = up_i(sAt_ptr, &D.At_ptr);
-    if (!rc) rc = up_i(sAt_idx, &D.At_idx);
-    if (!rc) rc = up_d(sAt_val, &D.At_val);
-    if (!rc) rc = up_i(sasm_ptr, &D.asm_ptr);
-    if (!rc) rc = up_i(sasm_col, &D.asm_col);
-    if (!rc) rc = up_d(sasm_val, &D.asm_val);
-    if (rc) return rc;
+    if (upload(Tm, ccnt, &D.ccnt) || upload(Tm, cnat, &D.cnat) || upload(Tm, sA_ptr, &D.A_ptr) || upload(Tm, sA_idx, &D.A_idx) ||
+        upload(Tm, sA_val, &D.A_val) || upload(Tm, sAt_ptr, &D.At_ptr) || upload(Tm, sAt_idx, &D.At_idx) ||
+        upload(Tm, sAt_val, &D.At_val) || upload(Tm, sasm_ptr, &D.asm_ptr) || upload(Tm, sasm_col, &D.asm_col) ||
+        upload(Tm, sasm_val, &D.asm_val))
+        return DSP_E_CUDA;
     D.Sr = Sr; D.Sc = Sc;
     D.ready = true;
     return 0;
@@ -1947,20 +1900,16 @@ static int launch_band_split(const dsp_template *T, KParams K, cudaStream_t st) 
     S.asm_ptr = D.asm_ptr; S.asm_col = D.asm_col; S.asm_val = D.asm_val;
     const int W = K.w;
     S.warp_doubles = (split_vec_doubles(D.Sr, D.Sc) + (long long)(2 * W + 1) * D.Sr * 32 + W * W * 32 + W * W + W + 31) / 32 * 32;
-    const size_t per_warp = (size_t)S.warp_doubles * sizeof(double);
     const BandSplitKernel kern = band_split_kernel(W);
     int occ = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32 * kSplitWarps, 0));
-    long long warps = std::min<long long>(K.N, (long long)T->sm_count * std::max(occ, 1) * kSplitWarps);
-    while (warps > 1 && (size_t)warps * per_warp > T->ws_cap) warps /= 2;
-    const int wpb = (int)std::min<long long>(kSplitWarps, std::max<long long>(1, warps / T->sm_count));
-    const long long blocks = (warps + wpb - 1) / wpb;
-    rc = grow_ws(T, (size_t)blocks * wpb * per_warp, st);
+    WsGrid g;
+    rc = ws_grid(T, K.N, (long long)T->sm_count * std::max(occ, 1) * kSplitWarps, kSplitWarps, (size_t)S.warp_doubles * sizeof(double), st, &g);
     if (rc) return rc;
     S.ws = T->ws;
     CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
-    kern<<<(unsigned)blocks, 32 * wpb, 0, st>>>(K, S);
-    rc = launched(blocks, 32 * wpb, 0, wpb);
+    kern<<<(unsigned)g.blocks, 32 * g.per_block, 0, st>>>(K, S);
+    rc = launched(g.blocks, 32 * g.per_block, 0, g.per_block);
     if (rc) return rc;
     // the LPs the split kernel leaves MAX_ITER / NUMERICAL get the band kernel's sequential elimination order (as behind the
     // long-horizon stage kernel)
@@ -1968,11 +1917,11 @@ static int launch_band_split(const dsp_template *T, KParams K, cudaStream_t st) 
     rc = launch_band(T, K, st);
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(g_mu);          // dsp_lp_last_launch reports the split kernel's geometry
-    g_last_grid = (int)blocks; g_last_block = 32 * wpb; g_last_smem = 0; g_last_ppc = wpb;
+    g_last_grid = (int)g.blocks; g_last_block = 32 * g.per_block; g_last_smem = 0; g_last_ppc = g.per_block;
     return 0;
 }
 
-// the dense kernels' data of a band template, built from its device copy of A at the first DSP_KERNEL_DENSE or _DENSE_CLUSTER call
+// the dense kernels' data of a band template, built from its host copy of A at the first DSP_KERNEL_DENSE or _DENSE_CLUSTER call
 static int ensure_dense(const dsp_template *T, bool cluster) {
     static std::mutex mu;
     std::lock_guard<std::mutex> lk(mu);
@@ -1985,12 +1934,7 @@ static int ensure_dense(const dsp_template *T, bool cluster) {
     }
     if (!cluster && K.m > kDenseMaxM) { g_err = "dsp_lp_solve_batch: DSP_KERNEL_DENSE needs m <= 1024 (m = " + std::to_string(K.m) + ")"; return DSP_E_ARG; }
     if (T->dn.ready) return 0;
-    std::vector<unsigned char> hot(K.hot_bytes);
-    CK(cudaMemcpy(hot.data(), K.hot_g, hot.size(), cudaMemcpyDeviceToHost));
-    const double *val = (const double *)hot.data();
-    const int *ptr = (const int *)(val + 2 * (size_t)K.nnz + K.nasm), *idx = ptr + K.m + 1;
-    return dense_build(const_cast<dsp_template *>(T), std::vector<int>(ptr, ptr + K.m + 1), std::vector<int>(idx, idx + K.nnz),
-                       std::vector<double>(val, val + K.nnz));
+    return dense_build(const_cast<dsp_template *>(T), T->band.A_ptr, T->band.A_idx, T->band.A_val);
 }
 
 // dense kernel: one persistent CTA per LP in flight, as many CTAs per SM as fit; the lower tiles of M of every CTA in the handle's
@@ -1999,15 +1943,11 @@ static DParams dense_params(const dsp_template *T, const KParams &K) {
     const dsp_template::Dense &D = T->dn;
     DParams Q;
     memset(&Q, 0, sizeof(Q));
-    Q.m = K.m; Q.n = K.n; Q.nb = K.nb; Q.Pc = K.Pc; Q.Pr = K.Pr; Q.nt = D.nt;
-    Q.c0 = K.c0; Q.b0 = K.b0; Q.u0 = K.u0; Q.omap = K.omap; Q.ocmap = K.ocmap;
-    Q.cm_ptr = K.cm_ptr; Q.cm_idx = K.cm_idx; Q.cm_val = K.cm_val; Q.bm_ptr = K.bm_ptr; Q.bm_idx = K.bm_idx; Q.bm_val = K.bm_val;
-    Q.um_ptr = K.um_ptr; Q.um_idx = K.um_idx; Q.um_val = K.um_val; Q.o0 = K.o0;
+    copy_batch(Q, K);
+    copy_maps(Q, K);
+    Q.nt = D.nt;
     Q.A_ptr = D.A_ptr; Q.A_idx = D.A_idx; Q.A_val = D.A_val; Q.At_ptr = D.At_ptr; Q.At_idx = D.At_idx; Q.At_val = D.At_val;
     Q.nent = D.nent; Q.asm_pos = D.asm_pos; Q.asm_ptr = D.asm_ptr; Q.asm_col = D.asm_col; Q.asm_val = D.asm_val;
-    Q.N = K.N; Q.cparams = K.cparams; Q.rparams = K.rparams; Q.rstride = K.rstride;
-    Q.tol = K.tol; Q.feas_tol = K.feas_tol; Q.step_frac = K.step_frac; Q.reg = K.reg; Q.max_iter = K.max_iter;
-    Q.obj = K.obj; Q.x_out = K.x_out; Q.y_out = K.y_out; Q.status = K.status; Q.iters = K.iters; Q.ticket = K.ticket;
     Q.xperm = K.xperm; Q.yperm = K.yperm;
     Q.nnz = K.nnz; Q.n_amq = D.n_amq; Q.nterms = D.nterms;
     Q.am_q = D.am_q; Q.am_ptr = D.am_ptr; Q.am_param = D.am_param; Q.am_coef = D.am_coef;
@@ -2016,6 +1956,8 @@ static DParams dense_params(const dsp_template *T, const KParams &K) {
 }
 
 static int launch_dense(const dsp_template *T, const KParams &K, cudaStream_t st) {
+    int rc = ensure_dense(T, false);
+    if (rc) return rc;
     const dsp_template::Dense &D = T->dn;
     DParams Q = dense_params(T, K);
     const bool per_lp = D.n_amq > 0;
@@ -2027,20 +1969,21 @@ static int launch_dense(const dsp_template *T, const KParams &K, cudaStream_t st
     void (*kern)(DParams) = per_lp ? dsp_ipm_dense_kernel<true> : dsp_ipm_dense_kernel<false>;
     int occ = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kDenseThreads, smem));
-    long long ctas = std::min<long long>(K.N, (long long)T->sm_count * std::max(occ, 1));
-    while (ctas > 1 && (size_t)ctas * Q.cta_doubles * 8 > T->ws_cap) ctas /= 2;
-    const int rc = grow_ws(T, (size_t)ctas * Q.cta_doubles * 8, st);
+    WsGrid g;
+    rc = ws_grid(T, K.N, (long long)T->sm_count * std::max(occ, 1), 1, (size_t)Q.cta_doubles * 8, st, &g);
     if (rc) return rc;
     Q.ws = T->ws;
     CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
-    kern<<<(unsigned)ctas, kDenseThreads, smem, st>>>(Q);
-    return launched(ctas, kDenseThreads, smem, 1);
+    kern<<<(unsigned)g.blocks, kDenseThreads, smem, st>>>(Q);
+    return launched(g.blocks, kDenseThreads, smem, 1);
 }
 
 // dense cluster kernel: one persistent cluster of C CTAs per LP in flight (C = 4 up to 32 tile rows, 8 above), as many clusters as
 // are co-resident; every cluster's region of the handle's workspace holds the LP's tiles, dinv and substitution vector, then each
 // rank's own per-LP vectors (when they do not fit in shared memory next to the staged-tile buffers) and matrix values (per-problem)
 static int launch_dense_cluster(const dsp_template *T, const KParams &K, cudaStream_t st) {
+    int rc = ensure_dense(T, true);
+    if (rc) return rc;
     const dsp_template::Dense &D = T->dn;
     DParams Q = dense_params(T, K);
     const bool per_lp = D.n_amq > 0;
@@ -2063,15 +2006,14 @@ static int launch_dense_cluster(const dsp_template *T, const KParams &K, cudaStr
     int ncl = 0;
     CK(cudaOccupancyMaxActiveClusters(&ncl, (void *)kern, &cfg));
     if (ncl < 1) { g_err = "dsp_lp_solve_batch: no cluster of " + std::to_string(csize) + " CTAs of the dense cluster kernel fits on the device"; return DSP_E_CUDA; }
-    long long clusters = std::min<long long>(K.N, ncl);
-    while (clusters > 1 && (size_t)clusters * Q.cta_doubles * 8 > T->ws_cap) clusters /= 2;
-    const int rc = grow_ws(T, (size_t)clusters * Q.cta_doubles * 8, st);
+    WsGrid g;
+    rc = ws_grid(T, K.N, ncl, 1, (size_t)Q.cta_doubles * 8, st, &g);
     if (rc) return rc;
     Q.ws = T->ws;
     CK(cudaMemsetAsync(K.ticket, 0, sizeof(unsigned long long), st));
-    cfg.gridDim = dim3((unsigned)(clusters * csize));
+    cfg.gridDim = dim3((unsigned)(g.blocks * csize));
     CK(cudaLaunchKernelEx(&cfg, kern, Q));
-    return launched(clusters * csize, kDenseThreads, smem, csize);
+    return launched(g.blocks * csize, kDenseThreads, smem, csize);
 }
 
 static int launch_batch(const dsp_template *T, int64_t N, const double *cparams, const double *rparams,
@@ -2085,6 +2027,8 @@ static int launch_batch(const dsp_template *T, int64_t N, const double *cparams,
     dsp_opts o;
     dsp_lp_default_opts(&o);
     if (opts) o = *opts;
+    Family f;
+    if (int rc = kernel_family(T, o.kernel, &f)) return rc;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     KParams K = T->kp;
     K.N = N; K.cparams = cparams; K.rparams = rparams; K.rstride = rparams_stride;
@@ -2092,45 +2036,23 @@ static int launch_batch(const dsp_template *T, int64_t N, const double *cparams,
     K.obj = obj; K.status = status; K.iters = iters; K.x_out = x; K.y_out = y;
     K.ticket = ticket;
     K.retry_only = 0;
-    if (T->cluster_only && o.kernel != DSP_KERNEL_AUTO && o.kernel != DSP_KERNEL_DENSE_CLUSTER) {
-        g_err = "dsp_lp_solve_batch: a template made by dsp_lp_template_create_dense_cluster runs only the dense cluster kernel (DSP_KERNEL_AUTO or DSP_KERNEL_DENSE_CLUSTER)";
-        return DSP_E_ARG;
+    switch (f) {
+        case F_DENSE_CLUSTER: return launch_dense_cluster(T, K, st);
+        case F_DENSE: return launch_dense(T, K, st);
+        case F_BAND_SPLIT: return launch_band_split(T, K, st);
+        case F_STAGE2_LONG:
+            if (int rc = launch_stage2_long(T, K, st)) return rc;
+            // At T = 8736 cond(M) reaches 1e15 and the partitioned elimination order rounds differently from the band kernel's
+            // sequential one: about 1 LP in 60 of the reference's full-year sweep stalls in the long kernel and converges in the
+            // band kernel.  The band kernel therefore follows on the same stream and re-solves ONLY the LPs the long kernel left
+            // with MAX_ITER / NUMERICAL (its warps skip every other ticket: a few microseconds when there is none).
+            K.retry_only = 1;
+            return launch_band(T, K, st);
+        case F_STAGE2: return launch_stage2(T, K, st);
+        case F_STAGE_V1: return launch_stage_v1(T, K, st);
+        case F_CHAIN1: return launch_chain1(T, K, st);
+        default: return launch_band(T, K, st);
     }
-    if (T->cluster_only || o.kernel == DSP_KERNEL_DENSE_CLUSTER) {
-        if (T->dense_only) { g_err = "dsp_lp_solve_batch: a template made by dsp_lp_template_create_dense runs only the dense kernel (DSP_KERNEL_AUTO or DSP_KERNEL_DENSE)"; return DSP_E_ARG; }
-        const int rc = ensure_dense(T, true);
-        if (rc) return rc;
-        return launch_dense_cluster(T, K, st);
-    }
-    if (T->dense_only && o.kernel != DSP_KERNEL_AUTO && o.kernel != DSP_KERNEL_DENSE) {
-        g_err = "dsp_lp_solve_batch: a template made by dsp_lp_template_create_dense runs only the dense kernel (DSP_KERNEL_AUTO or DSP_KERNEL_DENSE)";
-        return DSP_E_ARG;
-    }
-    if (T->dense_only || o.kernel == DSP_KERNEL_DENSE) {
-        const int rc = ensure_dense(T, false);
-        if (rc) return rc;
-        return launch_dense(T, K, st);
-    }
-    if (o.kernel == DSP_KERNEL_BAND_SPLIT) return launch_band_split(T, K, st);
-    const bool stage = o.kernel == DSP_KERNEL_AUTO || o.kernel == DSP_KERNEL_STAGE;
-    if (T->has_stage && T->sp.T > kStage2MaxT && stage) {
-        const int rc = launch_stage2_long(T, K, st);
-        if (rc) return rc;
-        // At T = 8736 cond(M) reaches 1e15 and the partitioned elimination order rounds differently from the band kernel's
-        // sequential one: about 1 LP in 60 of the reference's full-year sweep stalls in the long kernel and converges in the
-        // band kernel.  The band kernel therefore follows on the same stream and re-solves ONLY the LPs the long kernel left
-        // with MAX_ITER / NUMERICAL (its warps skip every other ticket: a few microseconds when there is none).
-        K.retry_only = 1;
-        return launch_band(T, K, st);
-    }
-    if (T->has_stage && stage) return launch_stage2(T, K, st);
-    if (T->has_stage && o.kernel == DSP_KERNEL_STAGE_V1) return launch_stage_v1(T, K, st);
-    if (T->has_chain1 && stage) return launch_chain1(T, K, st);
-    if (o.kernel == DSP_KERNEL_STAGE || o.kernel == DSP_KERNEL_STAGE_V1) {
-        g_err = "dsp_lp_solve_batch: the template has no stage descriptor";
-        return DSP_E_ARG;
-    }
-    return launch_band(T, K, st);
 }
 
 int dsp_lp_solve_batch(const dsp_template *T, int64_t N, const double *cparams, const double *rparams,
@@ -2190,26 +2112,7 @@ static int ensure_capacity(dsp_template *T, int64_t N, int64_t rp_rows, bool wan
 
 static int solve_batch_host_locked(dsp_template *T, int64_t N, const double *cparams, const double *rparams,
                                    int64_t rparams_stride, const dsp_opts *opts, double *obj, int32_t *status,
-                                   int32_t *iters, double *x, double *y);
-
-int dsp_lp_solve_batch_host(dsp_template *T, int64_t N, const double *cparams, const double *rparams,
-                            int64_t rparams_stride, const dsp_opts *opts, double *obj, int32_t *status,
-                            int32_t *iters, double *x, double *y) {
-    if (!T || N < 0) { g_err = "dsp_lp_solve_batch_host: bad arguments"; return DSP_E_ARG; }
-    int expected = 0;
-    if (!T->busy.compare_exchange_strong(expected, 1)) {       // not re-entrant per handle: enforced, not just documented
-        g_err = "dsp_lp_solve_batch_host: another host call is in flight on this template handle (use one handle per host thread)";
-        return DSP_E_BUSY;
-    }
-    const int rc = solve_batch_host_locked(T, N, cparams, rparams, rparams_stride, opts, obj, status, iters, x, y);
-    T->busy.store(0);
-    return rc;
-}
-
-static int solve_batch_host_locked(dsp_template *T, int64_t N, const double *cparams, const double *rparams,
-                                   int64_t rparams_stride, const dsp_opts *opts, double *obj, int32_t *status,
                                    int32_t *iters, double *x, double *y) {
-    if (!T || N < 0) { g_err = "dsp_lp_solve_batch_host: bad arguments"; return DSP_E_ARG; }
     if (N == 0) return 0;
     const KParams &K = T->kp;
     const int64_t rp_rows = (rparams_stride == 0) ? 1 : N;
@@ -2218,6 +2121,9 @@ static int solve_batch_host_locked(dsp_template *T, int64_t N, const double *cpa
         return DSP_E_ARG;
     }
     if (K.Pr > 0 && rparams_stride != 0 && rparams_stride < K.Pr) { g_err = "dsp_lp_solve_batch_host: rparams_stride < Pr"; return DSP_E_ARG; }
+    Family f;
+    int rc = kernel_family(T, opts ? opts->kernel : DSP_KERNEL_AUTO, &f);
+    if (rc) return rc;
     // chunked pipeline over two streams: the pinned-staging memcpy + H2D of chunk k+1 and the D2H of chunk k-1 overlap
     // the kernel of chunk k.  Caller buffers that are already page-locked (cudaHostAlloc / cudaHostRegister / a pinned
     // torch tensor) are used directly, without the staging copy (and without allocating staging buffers at all).
@@ -2229,19 +2135,20 @@ static int solve_batch_host_locked(dsp_template *T, int64_t N, const double *cpa
     };
     const bool in_pinned = pinned(cparams) && (K.Pr == 0 || pinned(rparams)) && (rparams_stride == 0 || rparams_stride == K.Pr);
     const bool out_pinned = pinned(obj) && pinned(status) && pinned(iters) && (!x || pinned(x)) && (!y || pinned(y));
-    int rc = ensure_capacity(T, N, rp_rows, x != nullptr, y != nullptr, !in_pinned, !out_pinned);
+    rc = ensure_capacity(T, N, rp_rows, x != nullptr, y != nullptr, !in_pinned, !out_pinned);
     if (rc) return rc;
     cudaStream_t sts[2] = {T->stream, T->stream2};
     int64_t dstride = 0;
-    // templates that run in global-workspace mode share ONE workspace: no concurrent chunk kernels for them
-    const bool dense = T->dense_only || T->cluster_only || (opts && (opts->kernel == DSP_KERNEL_DENSE || opts->kernel == DSP_KERNEL_DENSE_CLUSTER));    // the dense kernels always use the workspace
-    const bool ws_template = dense || band_geometry(T, K).ws || (T->has_stage && T->sp.T > kStage2MaxT);    // (the long stage kernel's workspace too)
+    // Kernels that run in the handle's ONE workspace take the batch in one chunk, so that no two chunk kernels share it: the split,
+    // long-horizon stage and dense kernels, and the band kernel in a workspace placement.  The other stage kernels of a template
+    // whose band kernel needs the workspace go in one chunk as well.
+    const bool one_ws = f == F_BAND_SPLIT || f == F_STAGE2_LONG || f == F_DENSE || f == F_DENSE_CLUSTER || band_geometry(T, K).ws;
     // Chunks pay when there is something to overlap: the staging memcpy of pageable input (always), or the H2D copy of a batch whose
     // kernel runs for many waves.  A page-locked batch of a few waves goes in ONE piece: the persistent stage kernels fill every SM
     // with one CTA, so two chunk kernels cannot share the chip and each chunk ends in its own thinning tail.
-    const int nchunk = ws_template ? 1
-                     : in_pinned   ? (int)std::min<int64_t>(4, std::max<int64_t>(1, N / 65536))
-                                   : (int)std::min<int64_t>(8, std::max<int64_t>(1, N / 2048));
+    const int nchunk = one_ws    ? 1
+                     : in_pinned ? (int)std::min<int64_t>(4, std::max<int64_t>(1, N / 65536))
+                                 : (int)std::min<int64_t>(8, std::max<int64_t>(1, N / 2048));
     const bool shared_rp = (K.Pr > 0 && rparams_stride == 0);
     if (shared_rp) {
         memcpy(T->h_rp, rparams, (size_t)K.Pr * 8);
@@ -2295,6 +2202,20 @@ static int solve_batch_host_locked(dsp_template *T, int64_t N, const double *cpa
         if (y) memcpy(y, T->h_y, (size_t)N * K.m * 8);
     }
     return 0;
+}
+
+int dsp_lp_solve_batch_host(dsp_template *T, int64_t N, const double *cparams, const double *rparams,
+                            int64_t rparams_stride, const dsp_opts *opts, double *obj, int32_t *status,
+                            int32_t *iters, double *x, double *y) {
+    if (!T || N < 0) { g_err = "dsp_lp_solve_batch_host: bad arguments"; return DSP_E_ARG; }
+    int expected = 0;
+    if (!T->busy.compare_exchange_strong(expected, 1)) {       // not re-entrant per handle: enforced, not just documented
+        g_err = "dsp_lp_solve_batch_host: another host call is in flight on this template handle (use one handle per host thread)";
+        return DSP_E_BUSY;
+    }
+    const int rc = solve_batch_host_locked(T, N, cparams, rparams, rparams_stride, opts, obj, status, iters, x, y);
+    T->busy.store(0);
+    return rc;
 }
 
 
@@ -2357,6 +2278,44 @@ std::vector<int> rcm_order(const std::vector<std::vector<int>> &adj) {
     return order;
 }
 
+// the internal column order of a standard-form LP: its bounded columns (u0 < 1e300) first, both groups in the caller's order
+std::vector<int> bounded_first(const dsp_lp_desc *D, int *nb) {
+    std::vector<int> col_perm;
+    for (int j = 0; j < D->n; ++j) if (D->u0[j] < 1e300) col_perm.push_back(j);
+    *nb = (int)col_perm.size();
+    for (int j = 0; j < D->n; ++j) if (!(D->u0[j] < 1e300)) col_perm.push_back(j);
+    return col_perm;
+}
+
+// pos[perm[k]] = k
+std::vector<int> inverse(const std::vector<int> &perm) {
+    std::vector<int> pos(perm.size());
+    for (size_t k = 0; k < perm.size(); ++k) pos[perm[k]] = (int)k;
+    return pos;
+}
+
+// D's matrix with rows in row_perm order and columns renumbered by col_pos, column indices sorted within every row
+void permute_csr(const dsp_lp_desc *D, const std::vector<int> &row_perm, const std::vector<int> &col_pos,
+                 std::vector<int> &A_ptr, std::vector<int> &A_idx, std::vector<double> &A_val) {
+    const int m = D->m;
+    A_ptr.assign(m + 1, 0); A_idx.resize(D->A_ptr[m]); A_val.resize(D->A_ptr[m]);
+    for (int k = 0; k < m; ++k) A_ptr[k + 1] = A_ptr[k] + (D->A_ptr[row_perm[k] + 1] - D->A_ptr[row_perm[k]]);
+    for (int k = 0; k < m; ++k) {
+        const int i = row_perm[k];
+        std::vector<std::pair<int, double>> ent;
+        for (int q = D->A_ptr[i]; q < D->A_ptr[i + 1]; ++q) ent.emplace_back(col_pos[D->A_idx[q]], D->A_val[q]);
+        std::sort(ent.begin(), ent.end());
+        for (size_t e = 0; e < ent.size(); ++e) { A_idx[A_ptr[k] + e] = ent[e].first; A_val[A_ptr[k] + e] = ent[e].second; }
+    }
+}
+
+// CSR position of the term (internal row i, internal column j), or -1 when it is not in the pattern
+int csr_pos(const std::vector<int> &A_ptr, const std::vector<int> &A_idx, int i, int j) {
+    int pos = -1;
+    for (int q = A_ptr[i]; q < A_ptr[i + 1]; ++q) if (A_idx[q] == j) pos = q;
+    return pos;
+}
+
 int analyze_csr(const dsp_lp_desc *D, CsrAnalysis &R) {
     if (!D || D->m <= 0 || D->n <= 0 || !D->A_ptr || !D->A_idx || !D->A_val || !D->u0) { g_err = "dsp_lp_analyze: bad descriptor"; return DSP_E_ARG; }
     const int m = D->m, n = D->n;
@@ -2364,12 +2323,7 @@ int analyze_csr(const dsp_lp_desc *D, CsrAnalysis &R) {
     for (int q = 0; q < nnz; ++q)
         if (D->A_idx[q] < 0 || D->A_idx[q] >= n) { g_err = "dsp_lp_analyze: A_idx out of range"; return DSP_E_ARG; }
     // 1. bounded columns first (stable)
-    R.col_perm.clear();
-    for (int j = 0; j < n; ++j) if (D->u0[j] < 1e300) R.col_perm.push_back(j);
-    R.nb = (int)R.col_perm.size();
-    for (int j = 0; j < n; ++j) if (!(D->u0[j] < 1e300)) R.col_perm.push_back(j);
-    std::vector<int> col_pos(n);
-    for (int k = 0; k < n; ++k) col_pos[R.col_perm[k]] = k;
+    R.col_perm = bounded_first(D, &R.nb);
     // 2. row graph of A A'
     std::vector<std::vector<int>> rows_of_col(n);
     for (int i = 0; i < m; ++i)
@@ -2388,18 +2342,8 @@ int analyze_csr(const dsp_lp_desc *D, CsrAnalysis &R) {
     R.w_rcm = bandwidth_of(adj, pos);
     R.row_perm = (R.w_natural <= R.w_rcm) ? nat : rcm;
     R.w = std::min(R.w_natural, R.w_rcm);
-    std::vector<int> row_pos(m);
-    for (int k = 0; k < m; ++k) row_pos[R.row_perm[k]] = k;
     // 3. permuted CSR with sorted column indices
-    R.A_ptr.assign(m + 1, 0); R.A_idx.resize(nnz); R.A_val.resize(nnz);
-    for (int k = 0; k < m; ++k) R.A_ptr[k + 1] = R.A_ptr[k] + (D->A_ptr[R.row_perm[k] + 1] - D->A_ptr[R.row_perm[k]]);
-    for (int k = 0; k < m; ++k) {
-        const int i = R.row_perm[k];
-        std::vector<std::pair<int, double>> ent;
-        for (int q = D->A_ptr[i]; q < D->A_ptr[i + 1]; ++q) ent.emplace_back(col_pos[D->A_idx[q]], D->A_val[q]);
-        std::sort(ent.begin(), ent.end());
-        for (size_t e = 0; e < ent.size(); ++e) { R.A_idx[R.A_ptr[k] + e] = ent[e].first; R.A_val[R.A_ptr[k] + e] = ent[e].second; }
-    }
+    permute_csr(D, R.row_perm, inverse(R.col_perm), R.A_ptr, R.A_idx, R.A_val);
     // 4. assembly list of the lower band of M = A D A':  M[i][i-k] = sum coef * d[col]   (coef = A[i][col] * A[i-k][col])
     const int w = R.w;
     struct Term { int col, qa, qb; double v; };
@@ -2430,6 +2374,32 @@ void permute_map(const dsp_param_map &in, const std::vector<int> &perm, int nrow
         ptr[k + 1] = (int)idx.size();
     }
 }
+
+// The internal descriptor d of a standard-form LP whose internal column k is caller column col_perm[k] (the first nb of them the
+// bounded ones) and internal row k caller row row_perm[k]: c0, b0, u0 and the parameter maps in that order, absent vectors as zeros.
+// The caller fills the matrix fields and w; d points into this object.
+struct StdForm {
+    std::vector<double> c0, b0, u0, zPr, zPc, cv, bv, uv;
+    std::vector<int> cp, ci, bp, bi, up, ui;
+    dsp_template_desc d;
+    StdForm(const dsp_lp_desc *D, const std::vector<int> &col_perm, int nb, const std::vector<int> &row_perm)
+        : c0(D->n), b0(D->m), u0(std::max(nb, 1)), zPr(std::max(D->Pr, 1), 0.0), zPc(std::max(D->Pc, 1), 0.0) {
+        const int m = D->m, n = D->n;
+        for (int k = 0; k < n; ++k) c0[k] = D->c0 ? D->c0[col_perm[k]] : 0.0;
+        for (int k = 0; k < nb; ++k) u0[k] = D->u0[col_perm[k]];
+        for (int k = 0; k < m; ++k) b0[k] = D->b0 ? D->b0[row_perm[k]] : 0.0;
+        permute_map(D->cmap, col_perm, n, cp, ci, cv);
+        permute_map(D->bmap, row_perm, m, bp, bi, bv);
+        permute_map(D->umap, col_perm, nb, up, ui, uv);
+        memset(&d, 0, sizeof(d));
+        d.m = m; d.n = n; d.nb = nb; d.Pc = D->Pc; d.Pr = D->Pr;
+        d.c0 = c0.data(); d.cmap.ptr = cp.data(); d.cmap.idx = ci.data(); d.cmap.val = cv.data();
+        d.b0 = b0.data(); d.bmap.ptr = bp.data(); d.bmap.idx = bi.data(); d.bmap.val = bv.data();
+        d.u0 = u0.data(); d.umap.ptr = up.data(); d.umap.idx = ui.data(); d.umap.val = uv.data();
+        d.o0 = D->o0; d.omap = D->omap ? D->omap : zPr.data(); d.ocmap = D->ocmap ? D->ocmap : zPc.data();
+    }
+    StdForm(const StdForm &) = delete;
+};
 }  // namespace
 
 int dsp_lp_analyze_csr(const dsp_lp_desc *D, int32_t *nb, int32_t *w, int32_t *w_natural, int32_t *w_rcm, int32_t *col_perm, int32_t *row_perm) {
@@ -2450,39 +2420,18 @@ int dsp_lp_template_create_csr(const dsp_lp_desc *D, dsp_template **out) {
     CsrAnalysis R;
     int rc = analyze_csr(D, R);
     if (rc) return rc;
-    const int m = D->m, n = D->n, nb = R.nb;
-    std::vector<double> c0(n), u0(std::max(nb, 1)), b0(m);
-    for (int k = 0; k < n; ++k) c0[k] = D->c0 ? D->c0[R.col_perm[k]] : 0.0;
-    for (int k = 0; k < nb; ++k) u0[k] = D->u0[R.col_perm[k]];
-    for (int k = 0; k < m; ++k) b0[k] = D->b0 ? D->b0[R.row_perm[k]] : 0.0;
-    std::vector<int> cp, ci, bp, bi, up, ui;
-    std::vector<double> cv, bv, uv;
-    permute_map(D->cmap, R.col_perm, n, cp, ci, cv);
-    permute_map(D->bmap, R.row_perm, m, bp, bi, bv);
-    permute_map(D->umap, R.col_perm, nb, up, ui, uv);
-    std::vector<double> zPr(std::max(D->Pr, 1), 0.0), zPc(std::max(D->Pc, 1), 0.0);
-    auto nz = [](std::vector<int> &v) { if (v.empty()) v.push_back(0); return v.data(); };
-    auto nzd = [](std::vector<double> &v) { if (v.empty()) v.push_back(0.0); return v.data(); };
-    dsp_template_desc d;
-    memset(&d, 0, sizeof(d));
-    d.m = m; d.n = n; d.nb = nb; d.w = R.w; d.Pc = D->Pc; d.Pr = D->Pr;
-    d.A_ptr = R.A_ptr.data(); d.A_idx = R.A_idx.data(); d.A_val = R.A_val.data();
-    d.asm_ptr = R.asm_ptr.data(); d.asm_col = nz(R.asm_col); d.asm_val = nzd(R.asm_val);
-    d.c0 = c0.data(); d.cmap.ptr = cp.data(); d.cmap.idx = nz(ci); d.cmap.val = nzd(cv);
-    d.b0 = b0.data(); d.bmap.ptr = bp.data(); d.bmap.idx = nz(bi); d.bmap.val = nzd(bv);
-    d.u0 = u0.data(); d.umap.ptr = up.data(); d.umap.idx = nz(ui); d.umap.val = nzd(uv);
-    d.o0 = D->o0; d.omap = D->omap ? D->omap : zPr.data(); d.ocmap = D->ocmap ? D->ocmap : zPc.data();
+    StdForm S(D, R.col_perm, R.nb, R.row_perm);
+    S.d.w = R.w;
+    S.d.A_ptr = R.A_ptr.data(); S.d.A_idx = R.A_idx.data(); S.d.A_val = R.A_val.data();
+    S.d.asm_ptr = R.asm_ptr.data(); S.d.asm_col = R.asm_col.data(); S.d.asm_val = R.asm_val.data();
     dsp_template *T = nullptr;
-    rc = dsp_lp_template_create(&d, &T);
+    rc = dsp_lp_template_create(&S.d, &T);
     if (rc) return rc;
+    Guard guard{T};
     T->col_perm = R.col_perm; T->row_perm = R.row_perm;
-    T->csr_ptr = R.A_ptr; T->csr_idx = R.A_idx; T->asm_qa = R.asm_qa; T->asm_qb = R.asm_qb;
-    int *dx = nullptr, *dy = nullptr;
-    rc = upload(R.col_perm, &dx);
-    if (!rc) { T->dev_allocs.push_back(dx); rc = upload(R.row_perm, &dy); }
-    if (rc) { dsp_lp_template_destroy(T); return rc; }
-    T->dev_allocs.push_back(dy);
-    T->kp.xperm = dx; T->kp.yperm = dy;
+    T->asm_qa = std::move(R.asm_qa); T->asm_qb = std::move(R.asm_qb);
+    if (upload(T, R.col_perm, &T->kp.xperm) || upload(T, R.row_perm, &T->kp.yperm)) return DSP_E_CUDA;
+    guard.t = nullptr;
     *out = T;
     return 0;
 }
@@ -2506,49 +2455,23 @@ static int create_dense(const char *fn, const dsp_lp_desc *D, int32_t count, con
     for (int q = 0; q < nnz; ++q)
         if (D->A_idx[q] < 0 || D->A_idx[q] >= n) { g_err = f + ": A_idx out of range"; return DSP_E_ARG; }
     // internal order: bounded columns first (stable), rows as given (the dense factorisation does not care about bandwidth)
-    std::vector<int> col_perm, row_perm(m);
-    for (int j = 0; j < n; ++j) if (D->u0[j] < 1e300) col_perm.push_back(j);
-    const int nb = (int)col_perm.size();
-    for (int j = 0; j < n; ++j) if (!(D->u0[j] < 1e300)) col_perm.push_back(j);
-    std::vector<int> col_pos(n);
-    for (int k = 0; k < n; ++k) col_pos[col_perm[k]] = k;
+    int nb;
+    const std::vector<int> col_perm = bounded_first(D, &nb), col_pos = inverse(col_perm);
+    std::vector<int> row_perm(m);
     for (int i = 0; i < m; ++i) row_perm[i] = i;
-    std::vector<int> A_ptr(m + 1, 0), A_idx(nnz);
-    std::vector<double> A_val(nnz);
-    std::vector<int> rmin(n, m), rmax(n, -1);
-    for (int i = 0; i < m; ++i) {
-        std::vector<std::pair<int, double>> ent;
-        for (int q = D->A_ptr[i]; q < D->A_ptr[i + 1]; ++q) {
-            const int j = col_pos[D->A_idx[q]];
-            ent.emplace_back(j, D->A_val[q]);
-            rmin[j] = std::min(rmin[j], i); rmax[j] = std::max(rmax[j], i);
-        }
-        std::sort(ent.begin(), ent.end());
-        A_ptr[i + 1] = A_ptr[i] + (int)ent.size();
-        for (size_t e = 0; e < ent.size(); ++e) { A_idx[A_ptr[i] + e] = ent[e].first; A_val[A_ptr[i] + e] = ent[e].second; }
-    }
+    std::vector<int> A_ptr, A_idx;
+    std::vector<double> A_val;
+    permute_csr(D, row_perm, col_pos, A_ptr, A_idx, A_val);
     int w = 0;                         // half bandwidth of A A' in this row order: rows sharing a column are adjacent
-    for (int j = 0; j < n; ++j) if (rmax[j] >= 0) w = std::max(w, rmax[j] - rmin[j]);
-    std::vector<double> c0(n), u0(std::max(nb, 1)), b0(m);
-    for (int k = 0; k < n; ++k) c0[k] = D->c0 ? D->c0[col_perm[k]] : 0.0;
-    for (int k = 0; k < nb; ++k) u0[k] = D->u0[col_perm[k]];
-    for (int i = 0; i < m; ++i) b0[i] = D->b0 ? D->b0[i] : 0.0;
-    std::vector<int> cp, ci, bp, bi, up, ui;
-    std::vector<double> cv, bv, uv;
-    permute_map(D->cmap, col_perm, n, cp, ci, cv);
-    permute_map(D->bmap, row_perm, m, bp, bi, bv);
-    permute_map(D->umap, col_perm, nb, up, ui, uv);
-    std::vector<double> zPr(std::max(D->Pr, 1), 0.0), zPc(std::max(D->Pc, 1), 0.0);
-    auto nz = [](std::vector<int> &v) { if (v.empty()) v.push_back(0); return v.data(); };
-    auto nzd = [](std::vector<double> &v) { if (v.empty()) v.push_back(0.0); return v.data(); };
-    dsp_template_desc d;
-    memset(&d, 0, sizeof(d));
-    d.m = m; d.n = n; d.nb = nb; d.w = w; d.Pc = D->Pc; d.Pr = D->Pr;
-    d.c0 = c0.data(); d.cmap.ptr = cp.data(); d.cmap.idx = nz(ci); d.cmap.val = nzd(cv);
-    d.b0 = b0.data(); d.bmap.ptr = bp.data(); d.bmap.idx = nz(bi); d.bmap.val = nzd(bv);
-    d.u0 = u0.data(); d.umap.ptr = up.data(); d.umap.idx = nz(ui); d.umap.val = nzd(uv);
-    d.o0 = D->o0; d.omap = D->omap ? D->omap : zPr.data(); d.ocmap = D->ocmap ? D->ocmap : zPc.data();
-    if (int rc = check_maps(&d)) return rc;
+    {
+        std::vector<int> rmin(n, m), rmax(n, -1);
+        for (int i = 0; i < m; ++i)
+            for (int q = A_ptr[i]; q < A_ptr[i + 1]; ++q) { rmin[A_idx[q]] = std::min(rmin[A_idx[q]], i); rmax[A_idx[q]] = i; }
+        for (int j = 0; j < n; ++j) if (rmax[j] >= 0) w = std::max(w, rmax[j] - rmin[j]);
+    }
+    StdForm S(D, col_perm, nb, row_perm);
+    S.d.w = w;
+    if (int rc = check_maps(&S.d)) return rc;
     // matrix terms: rows in the caller's order (kept), columns through col_pos, the entry must be in A's pattern
     if (count < 0 || (count > 0 && (!row || !col || !param || !coef))) { g_err = f + ": bad matrix parameter arguments"; return DSP_E_ARG; }
     DenseTerms terms;
@@ -2557,9 +2480,7 @@ static int create_dense(const char *fn, const dsp_lp_desc *D, int32_t count, con
             g_err = f + ": matrix parameter " + std::to_string(k) + " index out of range";
             return DSP_E_ARG;
         }
-        const int i = row[k], j = col_pos[col[k]];
-        int pos = -1;
-        for (int q = A_ptr[i]; q < A_ptr[i + 1]; ++q) if (A_idx[q] == j) pos = q;
+        const int pos = csr_pos(A_ptr, A_idx, row[k], col_pos[col[k]]);
         if (pos < 0) {
             g_err = f + ": matrix parameter " + std::to_string(k) + " is on an entry that is not in the sparsity pattern of A (store an explicit nominal value)";
             return DSP_E_ARG;
@@ -2567,20 +2488,13 @@ static int create_dense(const char *fn, const dsp_lp_desc *D, int32_t count, con
         terms.q.push_back(pos); terms.param.push_back(param[k]); terms.coef.push_back(coef[k]);
     }
     dsp_template *T = new dsp_template();
-    struct Guard {
-        dsp_template *t;
-        ~Guard() { if (t) dsp_lp_template_destroy(t); }
-    } guard{T};
-    if (int rc = template_init(T, &d)) return rc;
+    Guard guard{T};
+    if (int rc = template_init(T, &S.d)) return rc;
     T->kp.w = w; T->kp.nnz = nnz;
-    T->dense_only = !cluster;
-    T->cluster_only = cluster;
+    T->kind = cluster ? dsp_template::DENSE_CLUSTER : dsp_template::DENSE;
     if (int rc = dense_build(T, A_ptr, A_idx, A_val, &terms)) return rc;
     T->col_perm = col_perm; T->row_perm = row_perm;
-    int *dx = nullptr;
-    if (int rc = upload(col_perm, &dx)) return rc;
-    T->dev_allocs.push_back(dx);
-    T->kp.xperm = dx;                  // rows keep the caller's order: no y permutation
+    if (int rc = upload(T, col_perm, &T->kp.xperm)) return rc;     // rows keep the caller's order: no y permutation
     guard.t = nullptr;
     *out = T;
     return 0;
@@ -2603,43 +2517,27 @@ int dsp_lp_template_create_dense_cluster(const dsp_lp_desc *D, int32_t count, co
 int dsp_lp_template_set_matrix_params(dsp_template *T, int32_t count, const int32_t *row, const int32_t *col, const int32_t *param,
                                       const double *coef) {
     if (!T || count < 0 || (count > 0 && (!row || !col || !param || !coef))) { g_err = "dsp_lp_template_set_matrix_params: bad arguments"; return DSP_E_ARG; }
-    if (T->dense_only || T->cluster_only) { g_err = "dsp_lp_template_set_matrix_params: per-problem matrix coefficients are not supported on a dense template"; return DSP_E_ARG; }
-    if (T->csr_ptr.empty()) { g_err = "dsp_lp_template_set_matrix_params: the template must come from dsp_lp_template_create_csr"; return DSP_E_ARG; }
+    if (T->kind != dsp_template::BAND) { g_err = "dsp_lp_template_set_matrix_params: per-problem matrix coefficients are not supported on a dense template"; return DSP_E_ARG; }
+    if (T->col_perm.empty()) { g_err = "dsp_lp_template_set_matrix_params: the template must come from dsp_lp_template_create_csr"; return DSP_E_ARG; }
     if (T->kp.w != 1 && T->kp.w != 2 && T->kp.w != 4 && T->kp.w != 8 && T->kp.w != 16 && T->kp.w != 32) { g_err = "bad band"; return DSP_E_ARG; }
     KParams &K = T->kp;
     const int m = K.m, n = K.n, nnz = K.nnz;
-    std::vector<int> cpos(n), rpos(m);
-    for (int k = 0; k < n; ++k) cpos[T->col_perm[k]] = k;
-    for (int k = 0; k < m; ++k) rpos[T->row_perm[k]] = k;
+    const std::vector<int> cpos = inverse(T->col_perm), rpos = inverse(T->row_perm);
     std::vector<int> q(count), pr(count);
     std::vector<double> cf(count);
     for (int k = 0; k < count; ++k) {
         if (row[k] < 0 || row[k] >= m || col[k] < 0 || col[k] >= n || param[k] < 0 || param[k] >= K.Pr) { g_err = "matrix parameter index out of range"; return DSP_E_ARG; }
-        const int i = rpos[row[k]], j = cpos[col[k]];
-        int pos = -1;
-        for (int t = T->csr_ptr[i]; t < T->csr_ptr[i + 1]; ++t) if (T->csr_idx[t] == j) pos = t;
+        const int pos = csr_pos(T->band.A_ptr, T->band.A_idx, rpos[row[k]], cpos[col[k]]);
         if (pos < 0) { g_err = "matrix parameter on an entry that is not in the sparsity pattern of A (store an explicit nominal value)"; return DSP_E_ARG; }
         q[k] = pos; pr[k] = param[k]; cf[k] = coef[k];
     }
-    // CSC position -> CSR position: the same stable counting sort dsp_lp_template_create used for the values
-    std::vector<int> At_ptr(n + 1, 0), at_from(nnz);
-    for (int t = 0; t < nnz; ++t) At_ptr[T->csr_idx[t] + 1]++;
-    for (int j = 0; j < n; ++j) At_ptr[j + 1] += At_ptr[j];
-    {
-        std::vector<int> fill(At_ptr.begin(), At_ptr.end() - 1);
-        for (int i = 0; i < m; ++i)
-            for (int t = T->csr_ptr[i]; t < T->csr_ptr[i + 1]; ++t) at_from[fill[T->csr_idx[t]]++] = t;
-    }
-    int *dq, *dp, *daf, *dqa, *dqb; double *dc;
-    int rc = upload(q, &dq); if (rc) return rc; T->dev_allocs.push_back(dq);
-    rc = upload(pr, &dp); if (rc) return rc; T->dev_allocs.push_back(dp);
-    rc = upload(cf, &dc); if (rc) return rc; T->dev_allocs.push_back(dc);
-    rc = upload(at_from, &daf); if (rc) return rc; T->dev_allocs.push_back(daf);
-    rc = upload(T->asm_qa, &dqa); if (rc) return rc; T->dev_allocs.push_back(dqa);
-    rc = upload(T->asm_qb, &dqb); if (rc) return rc; T->dev_allocs.push_back(dqb);
+    const int *dq, *dp, *daf, *dqa, *dqb;
+    const double *dc;
+    if (upload(T, q, &dq) || upload(T, pr, &dp) || upload(T, cf, &dc) || upload(T, T->band.At.from, &daf) || upload(T, T->asm_qa, &dqa) ||
+        upload(T, T->asm_qb, &dqb))
+        return DSP_E_CUDA;
     if (K.n_amap == 0) { K.prob_doubles += 2 * nnz + K.nasm; K.band_doubles += 2 * nnz + K.nasm; }   // this LP's matrix values sit behind its band (in every placement)
     K.n_amap = count; K.amap_q = dq; K.amap_param = dp; K.amap_coef = dc; K.at_from = daf; K.asm_qa = dqa; K.asm_qb = dqb;
-    if (count == 0) K.n_amap = 0;
     return 0;
 }
 
