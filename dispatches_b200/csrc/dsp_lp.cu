@@ -1089,6 +1089,33 @@ inline Stage2Geom stage2_geometry(int T) {
 }
 constexpr int kStage2MaxT = 96;
 
+}  // namespace
+
+#include "dsp_sens.cuh"
+
+namespace {
+// sensitivity post-pass (dsp_sens.cuh): persistent CTAs of kSensWarps warps, one warp per LP, the template structure staged into
+// shared memory when it takes at most kSensSmemMax bytes
+constexpr int kSensWarps = 8;
+constexpr long long kSensSmemMax = 48 * 1024;
+__global__ void __launch_bounds__(32 * kSensWarps) dsp_lp_sens_kernel(const sens::Params P) {
+    extern __shared__ __align__(16) unsigned char sens_smem[];
+    const int lane = threadIdx.x & 31;
+    const long long nwarps = (long long)gridDim.x * kSensWarps;
+    const long long first = (long long)blockIdx.x * kSensWarps + (threadIdx.x >> 5);
+    if (P.blob_in_smem) {
+        const int4 *src = (const int4 *)P.blob;
+        int4 *dst = (int4 *)sens_smem;
+        for (long long k = threadIdx.x; k < P.L.bytes / 16; k += blockDim.x) dst[k] = __ldg(src + k);
+        __syncthreads();
+        const sens::View v = sens::view_of(sens_smem, P.L);
+        for (long long p = first; p < P.N; p += nwarps) sens::lp_body<false>(P, v, p, lane);
+    } else {
+        const sens::View v = sens::view_of(P.blob, P.L);
+        for (long long p = first; p < P.N; p += nwarps) sens::lp_body<true>(P, v, p, lane);
+    }
+}
+
 // FP64 FMA micro-benchmark: the measured denominator of the FP64 roofline fraction bench.py reports.  8 independent DFMA
 // chains per thread.
 __global__ void __launch_bounds__(256) dsp_fp64_peak_kernel(double *out, int iters, double a, double b) {
@@ -1161,11 +1188,26 @@ struct dsp_template {
     std::vector<void *> dev_allocs;
     std::vector<int> col_perm, row_perm;     // dsp_lp_template_create_csr / _dense: caller index of internal column / row
     std::vector<int> asm_qa, asm_qb;         // dsp_lp_template_create_csr: the two CSR positions of every assembly term
-    struct Band {                  // a band template's matrix in internal order: exactly what its hot blob packs
+    struct Band {                  // a band template's matrix in internal order: exactly what its hot blob packs (a dense template
+                                   // keeps only the CSR, for the sensitivity pass)
         std::vector<int> A_ptr, A_idx, asm_ptr, asm_col;    // CSR; band assembly list padded to half bandwidth kp.w
         std::vector<double> A_val, asm_val;
         Csc At;
     } band;
+    struct HostMaps {              // host copies of the parameter maps in internal order (umap: the first nb columns)
+        std::vector<double> c0, omap, ocmap, cm_val, bm_val, um_val;
+        std::vector<int> cm_ptr, cm_idx, bm_ptr, bm_idx, um_ptr, um_idx;
+    } maps;
+    struct Terms {                 // per-problem matrix terms in the caller's order: CSR position (internal order), rparams index, coef
+        std::vector<int> q, param;
+        std::vector<double> coef;
+    } mterms;
+    struct Sens {                  // the sensitivity pass's structure blob (built at the first dsp_lp_sensitivities call)
+        bool ready;
+        const unsigned char *blob;
+        sens::Layout L;
+    };
+    mutable Sens sns;
     unsigned long long *ticket;
     // host-call staging (pinned) and device buffers, grown on demand
     int64_t cap_N;
@@ -1312,6 +1354,14 @@ int template_init(dsp_template *T, const dsp_template_desc *D) {
         upload(T, D->umap.ptr, nb + 1, &K.um_ptr) || upload(T, D->umap.idx, D->umap.ptr[nb], &K.um_idx) ||
         upload(T, D->umap.val, D->umap.ptr[nb], &K.um_val))
         return DSP_E_CUDA;
+    dsp_template::HostMaps &H = T->maps;
+    H.c0.assign(D->c0, D->c0 + n); H.omap.assign(D->omap, D->omap + D->Pr); H.ocmap.assign(D->ocmap, D->ocmap + D->Pc);
+    H.cm_ptr.assign(D->cmap.ptr, D->cmap.ptr + n + 1); H.cm_idx.assign(D->cmap.idx, D->cmap.idx + D->cmap.ptr[n]);
+    H.cm_val.assign(D->cmap.val, D->cmap.val + D->cmap.ptr[n]);
+    H.bm_ptr.assign(D->bmap.ptr, D->bmap.ptr + m + 1); H.bm_idx.assign(D->bmap.idx, D->bmap.idx + D->bmap.ptr[m]);
+    H.bm_val.assign(D->bmap.val, D->bmap.val + D->bmap.ptr[m]);
+    H.um_ptr.assign(D->umap.ptr, D->umap.ptr + nb + 1); H.um_idx.assign(D->umap.idx, D->umap.idx + D->umap.ptr[nb]);
+    H.um_val.assign(D->umap.val, D->umap.val + D->umap.ptr[nb]);
     CK(cudaMalloc((void **)&T->ticket, 16 * sizeof(unsigned long long)));
     T->dev_allocs.push_back(T->ticket);
     CK(cudaStreamCreateWithFlags(&T->stream, cudaStreamNonBlocking));
@@ -2016,6 +2066,28 @@ static int launch_dense_cluster(const dsp_template *T, const KParams &K, cudaStr
     return launched(g.blocks * csize, kDenseThreads, smem, csize);
 }
 
+// The sensitivity pass's structure in the caller's column / row order (identity for dsp_lp_template_create): the CSC of A0, c0 and
+// Cmap by column, the transposed maps Cmap', Bmap', Umap' (bounded columns) by parameter, and the matrix terms grouped by column and
+// by parameter.  Every list runs in ascending caller index (matrix terms: in the caller's order within a group).  Built once per
+// handle, at the first dsp_lp_sensitivities call, and rebuilt after dsp_lp_template_set_matrix_params.
+static int ensure_sens(const dsp_template *T) {
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lk(mu);
+    if (T->sns.ready) return 0;
+    const KParams &K = T->kp;
+    const dsp_template::HostMaps &H = T->maps;
+    sens::HostTemplate S{K.m, K.n, K.nb, K.Pc, K.Pr, T->band.A_ptr, T->band.A_idx, T->band.A_val, T->col_perm, T->row_perm,
+                         H.c0, H.cm_ptr, H.cm_idx, H.cm_val, H.bm_ptr, H.bm_idx, H.bm_val, H.um_ptr, H.um_idx, H.um_val, H.omap, H.ocmap,
+                         T->mterms.q, T->mterms.param, T->mterms.coef};
+    std::vector<unsigned char> blob;
+    const sens::Layout L = sens::build_blob(S, blob);
+    dsp_template *Tm = const_cast<dsp_template *>(T);
+    if (int rc = upload(Tm, blob, &Tm->sns.blob)) return rc;
+    Tm->sns.L = L;
+    Tm->sns.ready = true;
+    return 0;
+}
+
 static int launch_batch(const dsp_template *T, int64_t N, const double *cparams, const double *rparams,
                         int64_t rparams_stride, const dsp_opts *opts, double *obj, int32_t *status, int32_t *iters,
                         double *x, double *y, void *cuda_stream, unsigned long long *ticket) {
@@ -2060,6 +2132,30 @@ int dsp_lp_solve_batch(const dsp_template *T, int64_t N, const double *cparams, 
                        double *x, double *y, void *cuda_stream) {
     return launch_batch(T, N, cparams, rparams, rparams_stride, opts, obj, status, iters, x, y, cuda_stream,
                         T ? T->ticket : nullptr);
+}
+
+int dsp_lp_sensitivities(const dsp_template *T, int64_t N, const double *cparams, const double *rparams, int64_t rparams_stride,
+                         const int32_t *status, const double *x, const double *y, double *rc, double *d_cparams, double *d_rparams,
+                         void *cuda_stream) {
+    if (!T) { g_err = "dsp_lp_sensitivities: null handle"; return DSP_E_ARG; }
+    if (N < 0) { g_err = "dsp_lp_sensitivities: N < 0"; return DSP_E_ARG; }
+    if (!status || !x || !y) { g_err = "dsp_lp_sensitivities: status, x and y are required (solve with x and y)"; return DSP_E_ARG; }
+    if (T->kp.Pc > 0 && !cparams) { g_err = "dsp_lp_sensitivities: cparams is NULL but the template has Pc > 0"; return DSP_E_ARG; }
+    if (T->kp.Pr > 0 && !rparams) { g_err = "dsp_lp_sensitivities: rparams is NULL but the template has Pr > 0"; return DSP_E_ARG; }
+    if (N == 0 || (!rc && !d_cparams && !d_rparams)) return 0;
+    if (int e = ensure_sens(T)) return e;
+    sens::Params P;
+    P.m = T->kp.m; P.n = T->kp.n; P.Pc = T->kp.Pc; P.Pr = T->kp.Pr;
+    P.N = N; P.cparams = cparams; P.rparams = rparams; P.rstride = rparams_stride;
+    P.status = status; P.x = x; P.y = y; P.rc = rc; P.dcp = d_cparams; P.drp = d_rparams;
+    P.blob = T->sns.blob; P.L = T->sns.L;
+    P.blob_in_smem = P.L.bytes <= kSensSmemMax;
+    const size_t smem = P.blob_in_smem ? (size_t)P.L.bytes : 0;
+    int occ = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dsp_lp_sens_kernel, 32 * kSensWarps, smem));
+    const long long blocks = std::min<long long>((N + kSensWarps - 1) / kSensWarps, (long long)T->sm_count * std::max(occ, 1));
+    dsp_lp_sens_kernel<<<(unsigned)blocks, 32 * kSensWarps, smem, (cudaStream_t)cuda_stream>>>(P);
+    return launched(blocks, 32 * kSensWarps, smem, kSensWarps);
 }
 
 static void free_staging(dsp_template *T) {
@@ -2493,6 +2589,8 @@ static int create_dense(const char *fn, const dsp_lp_desc *D, int32_t count, con
     T->kp.w = w; T->kp.nnz = nnz;
     T->kind = cluster ? dsp_template::DENSE_CLUSTER : dsp_template::DENSE;
     if (int rc = dense_build(T, A_ptr, A_idx, A_val, &terms)) return rc;
+    T->band.A_ptr = std::move(A_ptr); T->band.A_idx = std::move(A_idx); T->band.A_val = std::move(A_val);
+    T->mterms = {terms.q, terms.param, terms.coef};
     T->col_perm = col_perm; T->row_perm = row_perm;
     if (int rc = upload(T, col_perm, &T->kp.xperm)) return rc;     // rows keep the caller's order: no y permutation
     guard.t = nullptr;
@@ -2538,6 +2636,8 @@ int dsp_lp_template_set_matrix_params(dsp_template *T, int32_t count, const int3
         return DSP_E_CUDA;
     if (K.n_amap == 0) { K.prob_doubles += 2 * nnz + K.nasm; K.band_doubles += 2 * nnz + K.nasm; }   // this LP's matrix values sit behind its band (in every placement)
     K.n_amap = count; K.amap_q = dq; K.amap_param = dp; K.amap_coef = dc; K.at_from = daf; K.asm_qa = dqa; K.asm_qb = dqb;
+    T->mterms = {q, pr, cf};
+    T->sns.ready = false;          // the sensitivity pass rebuilds its structure with these terms
     return 0;
 }
 

@@ -348,7 +348,9 @@ def standard_form(rows, lo, hi, lb, ub, cost, c0=0.0, sense=1.0, var_names=None,
     # working representation: every model variable is  shift_j(p) + sign_j * y_{col_j}  [- y_{col2_j}] ; presolve may alias
     # variable i to variable j:  x_i = alpha * x_j + beta
     alias = {}                                        # i -> (j, alpha, beta0, dbeta[P])
+    elim = []                                         # (e, row, a_e, cost_e, dcost_e, {other live row: coef of e}), in elimination order
     rows = [dict(r) for r in rows]
+    model = dict(rows=[dict(r) for r in rows], cost=cvec.copy(), dcost=dcost.copy())
     live_row = np.ones(m, bool)
     if presolve:
         use = [set() for _ in range(n)]
@@ -379,6 +381,8 @@ def standard_form(rows, lo, hi, lb, ub, cost, c0=0.0, sense=1.0, var_names=None,
                         continue
                     # substitute x_e = alpha x_k + beta(p) everywhere
                     alias[e] = (k, alpha, beta, dhi[r] / ae)
+                    elim.append((e, r, ae, cvec[e], dcost[e].copy(),
+                                 {rr: rows[rr][e] for rr in use[e] if rr != r and live_row[rr] and e in rows[rr]}))
                     live_row[r] = False
                     for rr in list(use[e]):
                         if rr == r or not live_row[rr]:
@@ -481,7 +485,9 @@ def standard_form(rows, lo, hi, lb, ub, cost, c0=0.0, sense=1.0, var_names=None,
                    o_at_p0 - float(do @ p0) if P else o_at_p0, do.copy() * 0.0, do.copy(),
                    np.zeros(nc), np.ones(nc), names, [f"row[{i}]" for i in range(mr)],
                    dict(kind="standard_form", sense=sense))
-    t.meta["recover"] = dict(kind=kind, col=col, col2=col2, sgn=sgn, shift0=shift0, dshift=dshift, p0=p0, alias=alias, names=list(names))
+    t.meta["recover"] = dict(kind=kind, col=col, col2=col2, sgn=sgn, shift0=shift0, dshift=dshift, p0=p0, alias=alias, names=list(names),
+                             elim=elim)
+    t.meta["model"] = model
     t.meta["row_of"] = row_of
     t.meta["live_row"] = live_row
     # objective constant rides on ocmap (cparams) only: omap stays zero so that cparams == rparams does not count it twice
@@ -533,6 +539,29 @@ def model_duals(t: LPTemplate, y):
             k = pos[f"row[{mr}]"]
             out[:, r] = y[:, k] * (R[mr] if R is not None else 1.0) * t.meta["sense"]
     return out
+
+
+def model_reduced_costs(t: LPTemplate, y, params=None):
+    """Reduced costs of the model's variables [N, n_model] of a standard_form() template from its row duals y [N, m]:
+    rc = c_model(params) - A_model' y_model, in the model's own objective sense, with y_model the duals of model_duals() and, for the rows
+    presolve removed, the duals that make each eliminated variable's reduced cost 0 (solved back in reverse elimination order; a free
+    variable has reduced cost 0 at every optimum, and for a variable merged with an identically bounded one that choice leaves the
+    bound multipliers on the one kept).  Fixed, flipped, split and presolved variables are then covered by the definition itself."""
+    rec, mdl = t.meta["recover"], t.meta["model"]
+    ym = model_duals(t, y)
+    N, n = ym.shape[0], rec["kind"].size
+    P = rec["p0"].size
+    dp = (np.atleast_2d(params) - rec["p0"]) if (params is not None and P) else np.zeros((N, P))
+    for e, r, ae, ce, dce, others in reversed(rec["elim"]):
+        c_e = ce + (dp @ dce if P else 0.0)
+        ym[:, r] = (c_e - sum(a * ym[:, rr] for rr, a in others.items())) / ae
+    ri, ci, vv = [], [], []
+    for r, row in enumerate(mdl["rows"]):
+        for j, a in row.items():
+            ri.append(r); ci.append(j); vv.append(a)
+    A = sp.csr_matrix((vv, (ri, ci)), shape=(len(mdl["rows"]), n))
+    c = mdl["cost"][None, :] + (dp @ mdl["dcost"].T if P else 0.0)
+    return c - (A.T @ ym.T).T
 
 
 # ----------------------------------------------------------------------------------------------------------------------

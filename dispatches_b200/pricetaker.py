@@ -22,7 +22,7 @@ import dataclasses
 import numpy as np
 
 from . import templates as TP
-from .solver import KERNEL_DENSE, KERNEL_DENSE_CLUSTER, BatchLPSolver, OPTIMAL, STATUS_NAMES
+from .solver import KERNEL_DENSE, KERNEL_DENSE_CLUSTER, BatchLPSolver, LPResult, OPTIMAL, STATUS_NAMES
 
 _SOLVERS = {}
 
@@ -59,6 +59,12 @@ class PriceTakerResult:
     x: np.ndarray | None            # [N,n] model-space values of the template columns
     col_names: list
     sizes: dict
+    # want_sensitivities=True (renewables cases): d NPV / d (size in MW, h2 price in $/kg, LMP in $/MWh), [N] arrays ([N,T] for
+    # "lmp"); NPV = -1e5 obj.  Where an LP's optimum is not unique the values are a supergradient / subgradient of the NPV
+    # (include/dsp_lp.h: dsp_lp_sensitivities).
+    marginal_npv: dict | None = None
+    # want_sensitivities=True (nuclear case, whose objective is an operating cost, not -1e-5 NPV): d obj / d LMP [N,T] under "lmp"
+    marginal_obj: dict | None = None
 
     @property
     def NPV(self):
@@ -117,11 +123,35 @@ def _lmps(input_params, T):
     return np.ascontiguousarray(lmp)
 
 
-def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solution=True, kernel=None):
+def _solve_with_sensitivities(sol, cp, rp):
+    """the batch through the device path (dsp_lp_solve_batch with x and y, then dsp_lp_sensitivities) on cuda:0; numpy results"""
+    import torch
+    dev = torch.device("cuda", 0)
+    cpt = torch.as_tensor(np.ascontiguousarray(cp, float), device=dev)
+    rpt = torch.as_tensor(np.ascontiguousarray(rp, float), device=dev) if rp is not None else None
+    r = sol.solve(cpt, rpt, want_x=True, want_y=True)
+    g = sol.sensitivities(cpt, rpt, r, want_rc=False)
+    host = lambda a: a.cpu().numpy()
+    return LPResult(host(r.obj), host(r.status), host(r.iters), host(r.x), host(r.y)), host(g.d_cparams), host(g.d_rparams)
+
+
+def _wind_marginals(T, cf, dc, dr, N, pem=False):
+    """d NPV / d sizes and prices of wind_battery(_pem): rparams = [wind_kw cf_t (T), batt_kw, wind_kw(, pem_kw)], cparams = [lmp(, h2)]"""
+    cf = np.broadcast_to(np.asarray(cf, float), (N, T))
+    out = dict(wind_mw=-1e5 * 1e3 * ((cf * dr[:, :T]).sum(1) + dr[:, T + 1]), batt_mw=-1e5 * 1e3 * dr[:, T], lmp=-1e5 * dc[:, :T])
+    if pem:
+        out.update(pem_mw=-1e5 * 1e3 * dr[:, T + 2], h2_price_per_kg=-1e5 * dc[:, T])
+    return out
+
+
+def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solution=True, kernel=None, want_sensitivities=False):
     """kernel: a solver.KERNEL_* choice for the band-template paths (None: the library's default, e.g. KERNEL_BAND_SPLIT for a long
-    horizon on the split band kernel); the free-wind design (per-problem matrix coefficients) does not take it"""
+    horizon on the split band kernel); the free-wind design (per-problem matrix coefficients) does not take it.
+    want_sensitivities (fixed design only): fill PriceTakerResult.marginal_npv (wind_mw, batt_mw, lmp)."""
     T = int(n_time_points)
     design = bool(input_params.get("design_opt", False))
+    if want_sensitivities and design:
+        raise NotImplementedError("want_sensitivities needs a fixed design (design_opt=False)")
     lmp = _lmps(input_params, T)
     cf = _capacity_factors(input_params, T)
     if design and not input_params.get("extant_wind", True):
@@ -134,7 +164,12 @@ def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solut
         rp = rp[0]
     elif rp.shape[0] != lmp.shape[0]:
         raise ValueError("sizes / capacity factors must be scalar or match the number of LMP scenarios")
-    r = sol.solve_host(lmp, rp, want_x=want_solution)
+    marginal = None
+    if want_sensitivities:
+        r, dc, dr = _solve_with_sensitivities(sol, lmp, rp)
+        marginal = _wind_marginals(T, cf, dc, dr, lmp.shape[0])
+    else:
+        r = sol.solve_host(lmp, rp, want_x=want_solution)
     if verbose:
         print(f"b200ipm: {lmp.shape[0]} LPs, iterations mean {r.iters.mean():.1f} max {r.iters.max()}, "
               f"non-optimal {(r.status != OPTIMAL).sum()}")
@@ -144,7 +179,7 @@ def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solut
     xm = sol.to_model_space(r.x) if want_solution else None
     if design:                                        # optimised size: value(m.battery_system_capacity)
         sizes["batt_kw"] = xm[:, sol.t.col_names.index("blk[0].fs.battery.nameplate_power")].copy()
-    return PriceTakerResult("wind_battery", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes)
+    return PriceTakerResult("wind_battery", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes, marginal)
 
 
 def _wind_battery_free_wind(T, lmp, cf, input_params, verbose):
@@ -181,9 +216,12 @@ def _wind_battery_free_wind(T, lmp, cf, input_params, verbose):
     return PriceTakerResult("wind_battery", T, lmp, r.obj, r.status, r.iters, xm, names, sizes)
 
 
-def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_solution=True, kernel=None):
-    """kernel: a solver.KERNEL_* choice (None: the library's default)"""
+def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_solution=True, kernel=None, want_sensitivities=False):
+    """kernel: a solver.KERNEL_* choice (None: the library's default).  want_sensitivities (fixed design only): fill
+    PriceTakerResult.marginal_npv (wind_mw, batt_mw, pem_mw, h2_price_per_kg, lmp)."""
     mode = input_params.get("design_opt", False)
+    if want_sensitivities and mode is not False:
+        raise NotImplementedError("want_sensitivities needs a fixed design (design_opt=False)")
     if mode not in (False, "PEM") or (mode == "PEM" and not input_params.get("extant_wind", True)):
         raise NotImplementedError("only design_opt False and \"PEM\" (extant wind) are on the batched GPU path")
     pem_design = mode == "PEM"
@@ -192,7 +230,9 @@ def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_sol
     N = lmp.shape[0]
     cf = _capacity_factors(input_params, T)
     batt = np.zeros(1) if pem_design else np.asarray(input_params["batt_mw"], float)   # "PEM" fixes the battery at 0 (:228)
-    with_batt = bool(np.any(batt > 0))
+    # without a battery the template drops its columns; the sensitivities keep them (bounded by a zero size through Umap), so that
+    # d NPV / d batt_mw at 0 is the value of the first MW of battery, not only its cost
+    with_batt = bool(np.any(batt > 0)) or want_sensitivities
     want_solution = want_solution or pem_design
     sol = get_solver("wind_battery_pem", T, kernel=kernel, with_battery=with_batt, extant_wind=bool(input_params.get("extant_wind", True)),
                      pem_design=pem_design)
@@ -203,24 +243,35 @@ def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_sol
         raise ValueError("sizes / capacity factors must be scalar or match the number of LMP scenarios")
     h2 = np.broadcast_to(np.asarray(input_params["h2_price_per_kg"], float), (N,))
     cp = np.ascontiguousarray(np.concatenate([lmp, h2[:, None]], axis=1))
-    r = sol.solve_host(cp, rp, want_x=want_solution)
+    marginal = None
+    if want_sensitivities:
+        r, dc, dr = _solve_with_sensitivities(sol, cp, rp)
+        marginal = _wind_marginals(T, cf, dc, dr, N, pem=True)
+    else:
+        r = sol.solve_host(cp, rp, want_x=want_solution)
     sizes = dict(wind_kw=np.broadcast_to(np.asarray(input_params["wind_mw"], float) * 1e3, (N,)),
                  batt_kw=np.broadcast_to(batt * 1e3, (N,)),
                  pem_kw=np.broadcast_to(np.asarray(input_params["pem_mw"], float) * 1e3, (N,)), h2_price=h2)
     xm = sol.to_model_space(r.x) if want_solution else None
     if pem_design:                                    # optimised size: value(m.pem_system_capacity)
         sizes["pem_kw"] = xm[:, sol.t.col_names.index("pem_system_capacity[0]")].copy()
-    return PriceTakerResult("wind_battery_pem", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes)
+    return PriceTakerResult("wind_battery_pem", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes, marginal)
 
 
-def nuclear_dispatch_optimize(n_time_points, lmps, want_solution=False, kernel=None, **flowsheet_options):
-    """kernel: a solver.KERNEL_* choice (None: the library's default)"""
+def nuclear_dispatch_optimize(n_time_points, lmps, want_solution=False, kernel=None, want_sensitivities=False, **flowsheet_options):
+    """kernel: a solver.KERNEL_* choice (None: the library's default).  want_sensitivities: fill PriceTakerResult.marginal_obj["lmp"]
+    = d obj / d lmp [N,T] (the sizes are template constants, not parameters)."""
     T = int(n_time_points)
     lmp = np.ascontiguousarray(np.atleast_2d(np.asarray(lmps, float))[:, :T])
     sol = get_solver("nuclear", T, kernel=kernel, **flowsheet_options)
-    r = sol.solve_host(lmp, None, want_x=want_solution)
+    marginal = None
+    if want_sensitivities:
+        r, dc, _ = _solve_with_sensitivities(sol, lmp, None)
+        marginal = dict(lmp=dc[:, :T])
+    else:
+        r = sol.solve_host(lmp, None, want_x=want_solution)
     return PriceTakerResult("nuclear", T, lmp, r.obj, r.status, r.iters,
-                            sol.to_model_space(r.x) if want_solution else None, sol.t.col_names, {})
+                            sol.to_model_space(r.x) if want_solution else None, sol.t.col_names, {}, marginal_obj=marginal)
 
 
 _SOLAR_COST_KEYS = ("pv_cap_cost", "pv_op_cost", "batt_cap_cost_kw", "batt_cap_cost_kwh", "pem_cap_cost", "pem_op_cost", "pem_var_cost",

@@ -15,8 +15,8 @@ from __future__ import annotations
 
 import numpy as np
 
-from .lp_template import INF, model_duals, model_values, standard_form
-from .solver import INFEASIBLE, MAX_ITER, OPTIMAL, BatchLPSolver
+from .lp_template import INF, model_duals, model_reduced_costs, model_values, standard_form
+from .solver import INFEASIBLE, MAX_ITER, OPTIMAL, BatchLPSolver, LPResult
 
 try:                                            # pragma: no cover - pyomo absent in the build image
     import pyomo.environ as pyo
@@ -109,8 +109,10 @@ def walk_model(model, batch_params=None):
 
 class B200IPM:
     """Object with the part of Pyomo's solver interface the reference uses (SURVEY.md 8b): ``available()``, ``options``,
-    ``solve(model, tee=...)`` writing Var values (and ``model.dual`` when the model declares an IMPORT Suffix of that name) back,
-    returning SolverResults with solver.status / termination_condition."""
+    ``solve(model, tee=...)`` writing Var values (and ``model.dual`` / ``model.rc`` when the model declares an IMPORT Suffix of that
+    name) back, returning SolverResults with solver.status / termination_condition.  ``options={"sensitivities": True}`` adds
+    ``res.batch["d_params"]`` [N, P]: d objective / d every batched Param (a subgradient where the optimum is not unique), from the
+    GPU post-pass dsp_lp_sensitivities."""
 
     def __init__(self, **kw):
         self.options = dict(tol=1e-9, feas_tol=1e-9, max_iter=60)
@@ -138,8 +140,19 @@ class B200IPM:
             pv = np.column_stack([np.asarray(batch_params[p], float) for p in batch_params])
         else:
             pv = p0[None, :] if p0.size else np.zeros((1, 0))
-        r = sol.solve_host(pv, pv if t.Pr else None, want_x=True, want_y=True)
         sense = t.meta["sense"]
+        d_params = None
+        if opts.get("sensitivities"):
+            # the device path: the same Param vector is cparams and rparams, so d obj / d Param = d_cparams + d_rparams
+            import torch
+            dev = torch.device("cuda", torch.cuda.current_device())
+            pvt = torch.as_tensor(np.ascontiguousarray(pv, float), device=dev)
+            rd = sol.solve(pvt, pvt if t.Pr else None, want_x=True, want_y=True)
+            g = sol.sensitivities(pvt, pvt if t.Pr else None, rd, want_rc=False)
+            d_params = sense * (g.d_cparams + g.d_rparams).cpu().numpy()
+            r = LPResult(*(a.cpu().numpy() for a in (rd.obj, rd.status, rd.iters, rd.x, rd.y)))
+        else:
+            r = sol.solve_host(pv, pv if t.Pr else None, want_x=True, want_y=True)
         xm = model_values(t, r.x, pv)
         ym = model_duals(t, r.y)
         if pv.shape[0] == 1:                    # plain solver behaviour: write back into the Vars (and the dual Suffix)
@@ -150,6 +163,11 @@ class B200IPM:
             if dual is not None and hasattr(dual, "import_enabled") and dual.import_enabled():
                 for i, c in enumerate(cons):
                     dual[c] = float(ym[0, i])
+            rc = getattr(model, "rc", None)
+            if rc is not None and hasattr(rc, "import_enabled") and rc.import_enabled():
+                rcm = model_reduced_costs(t, r.y, pv)
+                for j, v in enumerate(vars_):
+                    rc[v] = float(rcm[0, j])
         res = SolverResults()
         worst = int(r.status.max())
         res.solver.status = {OPTIMAL: SolverStatus.ok, MAX_ITER: SolverStatus.warning}.get(worst, SolverStatus.error)
@@ -157,6 +175,8 @@ class B200IPM:
                                             INFEASIBLE: TerminationCondition.infeasible}.get(worst, TerminationCondition.error)
         res.problem.lower_bound = res.problem.upper_bound = float(sense * r.obj[0])
         res.batch = dict(obj=sense * r.obj, status=r.status, iters=r.iters, x=xm, duals=ym, var_names=[v.name for v in vars_])
+        if d_params is not None:
+            res.batch["d_params"] = d_params
         if tee:
             print(f"b200ipm: {pv.shape[0]} LP(s), m={t.m} n={t.n} w={t.w}, iterations max {int(r.iters.max())}")
         return res

@@ -217,6 +217,26 @@ int dsp_lp_solve_batch_host(dsp_template *t, int64_t N,
                             const dsp_opts *opts,
                             double *obj, int32_t *status, int32_t *iters, double *x, double *y);
 
+/* Sensitivities of a solved batch: reduced costs and the objective's derivative in every batch parameter, a post-pass over the
+ * (status, x, y) that dsp_lp_solve_batch returned for the same cparams / rparams.  For one LP with returned (x, y):
+ *     rc            = c - A'y            A: the LP's own matrix, A0 + sum coef * rparams[param] (per-problem matrix terms)
+ *     d obj / d cp  = Cmap' x + ocmap
+ *     d obj / d rp  = Bmap' y + Umap' min(rc, 0) + omap - sum over the matrix terms (i, j, q, coef) of coef * y_i * x_j
+ * min(rc_j, 0) is minus the upper-bound dual that is optimal for this y.  Where the optimum is unique these are the gradient of the
+ * optimal value obj = c'x + k (envelope theorem); at a degenerate optimum they are a subgradient: obj is convex in rparams when rparams
+ * does not enter A, and concave in cparams.
+ * DEVICE pointers, stream-ordered, no synchronisation, like dsp_lp_solve_batch (the same rparams_stride == 0 broadcast); x [N,n], y [N,m],
+ * rc [N,n], d_cparams [N,Pc], d_rparams [N,Pr] in the same (caller's) order as dsp_lp_solve_batch's x and y.  Each output may be NULL; an
+ * LP whose status is not DSP_OPTIMAL gets rows of NaN in every requested output.  Every entry is summed in a fixed order by one thread:
+ * the results are bitwise reproducible and do not depend on where an LP sits in the batch.  One kernel launch per call (none when
+ * N == 0 or every output is NULL); the first call on a handle builds its structure on the host.
+ * DSP_E_ARG: NULL handle, N < 0, NULL status / x / y, NULL cparams with Pc > 0 or NULL rparams with Pr > 0. */
+int dsp_lp_sensitivities(const dsp_template *t, int64_t N,
+                         const double *cparams, const double *rparams, int64_t rparams_stride,
+                         const int32_t *status, const double *x, const double *y,
+                         double *rc /*[N,n] or NULL*/, double *d_cparams /*[N,Pc] or NULL*/, double *d_rparams /*[N,Pr] or NULL*/,
+                         void *cuda_stream);
+
 /* Introspection used by tests / bench: kernel launches issued so far, last launch geometry (grid in CTAs, block, dynamic shared
  * memory; problems_per_cta: LPs per CTA, or for the dense cluster kernel the cluster size in CTAs). */
 int64_t dsp_lp_launch_count(void);
