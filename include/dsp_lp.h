@@ -69,10 +69,13 @@ typedef struct {
     double  tol;          /* relative duality-gap tolerance (default 1e-9)              */
     double  feas_tol;     /* relative primal / dual residual tolerance (default 1e-9)   */
     int32_t max_iter;     /* default 60                                                  */
-    double  step_frac;    /* fraction of the step to the boundary (default 0.9995)       */
+    double  step_frac;    /* fraction of the step to the boundary (default 0.9995), first attempt only (see below) */
     int32_t device;       /* reserved (the current CUDA device is used); keep -1        */
     double  reg_primal;   /* proximal regularisation of D^-1 in scaled units (default 1e-8; applied as reg/max(1,x^2)): caps the scaling
-                             of never-binding columns (throughput, slacks) so A D A' stays factorisable    */
+                             of never-binding columns (throughput, slacks) so A D A' stays factorisable.  First attempt only:
+                             an LP whose first attempt ends MAX_ITER or NUMERICAL is solved again from the start point with
+                             step_frac = 0.99 and 10 x reg_primal (100 x in the long-horizon stage kernel and in
+                             DSP_KERNEL_BAND_SPLIT), and iters counts both attempts    */
     int32_t kernel;       /* DSP_KERNEL_AUTO (stage kernel when the template has one), _BAND, _STAGE, _STAGE_V1 */
 } dsp_opts;
 

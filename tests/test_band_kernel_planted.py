@@ -46,21 +46,21 @@ def _assert_full_launch(p, pl, warps):
     assert ll["grid"] == _sms() and ll["block"] == 32 * warps and warps > 1, (ll, warps)
 
 
-def _solver(p, native):
+def _solver(p, native, **opts):
     if native:
         t, cperm, rperm = shuffled(p.t, seed=7)
-        return S.BatchLPSolver(t, native_setup=True), cperm, rperm
-    return S.BatchLPSolver(p.t), None, None
+        return S.BatchLPSolver(t, native_setup=True, **opts), cperm, rperm
+    return S.BatchLPSolver(p.t, **opts), None, None
 
 
-def _check(p, r, cperm=None, rperm=None, what=""):
-    """status, objective within OBJ_REL of the exact optimum, x / y within XY_REL of the planted ones (caller order); returns the
-    largest (objective, x, y) errors"""
+def _check(p, r, cperm=None, rperm=None, what="", obj_rel=OBJ_REL):
+    """status, objective within obj_rel (default OBJ_REL) of the exact optimum, x / y within XY_REL of the planted ones (caller
+    order); returns the largest (objective, x, y) errors"""
     assert (r.status == S.OPTIMAL).all(), (what, r.status, r.iters)
     eo = np.abs(r.obj - p.obj) / np.maximum(1.0, np.abs(p.obj))
-    assert eo.max() <= OBJ_REL, (what, eo.max())
+    assert eo.max() <= obj_rel, (what, eo.max())
     el = np.abs(r.obj - p.obj)[p.lp_mag > 0] / p.lp_mag[p.lp_mag > 0]
-    assert el.max(initial=0.0) <= OBJ_REL, (what, "LP part", el.max())
+    assert el.max(initial=0.0) <= obj_rel, (what, "LP part", el.max())
     x = p.x if cperm is None else p.x[:, cperm]
     y = p.y if rperm is None else p.y[:, rperm]
     ex = ey = 0.0

@@ -61,15 +61,16 @@ def _units(t, s, kernel):
     return ll["grid"] // ll["problems_per_cta"]
 
 
-def _run(s, name, kernel, t=None, cperm=None, rperm=None):
-    """s through one dense kernel, on s.t or on ``t``, the same LPs with column j / row i being column cperm[j] / row rperm[i] of
-    s.t; on the cluster kernel at m <= 1024 also through the single-CTA kernel, which must give the same bits"""
+def _run(s, name, kernel, t=None, cperm=None, rperm=None, opts={}):
+    """s through one dense kernel with solver options ``opts``, on s.t or on ``t``, the same LPs with column j / row i being column
+    cperm[j] / row rperm[i] of s.t; on the cluster kernel at m <= 1024 also through the single-CTA kernel, which must give the same
+    bits.  Returns the tiled set and the result."""
     t = s.t if t is None else t
     units = _units(t, s, kernel)
     N = 2 * units + 5
     q, k = s.tile(N, seed=1)
     rp = q.rparams if t.Pr else None
-    r = S.BatchLPSolver(t, kernel=KERNELS[kernel]).solve_host(q.cparams, rp, want_x=True, want_y=True)
+    r = S.BatchLPSolver(t, kernel=KERNELS[kernel], **opts).solve_host(q.cparams, rp, want_x=True, want_y=True)
     ll = S.last_launch()
     ppc = 1 if kernel == "dense" else _cluster_size(t.m)
     assert ll["block"] == THREADS and ll["problems_per_cta"] == ppc and ll["grid"] == ppc * units and units < N, ll
@@ -84,13 +85,13 @@ def _run(s, name, kernel, t=None, cperm=None, rperm=None):
     e = R.check_exact(q, r.obj, r.status, r.x, r.y, cperm=cperm, rperm=rperm, kkt_rows=first, what=name)
     same = ""
     if kernel == "cluster" and t.m <= MAX_M["dense"]:
-        d = S.BatchLPSolver(t, kernel=S.KERNEL_DENSE).solve_host(q.cparams, rp, want_x=True, want_y=True)
+        d = S.BatchLPSolver(t, kernel=S.KERNEL_DENSE, **opts).solve_host(q.cparams, rp, want_x=True, want_y=True)
         for what in ("status", "obj", "iters", "x", "y"):
             assert np.array_equal(getattr(r, what), getattr(d, what)), (name, what, "differs from the single-CTA kernel")
         same = ", bitwise the single-CTA kernel's"
     print(f"{name} on the {kernel} kernel: m = {t.m}, {N} LPs{placement}, iters mean {r.iters.mean():.1f} max {r.iters.max()}{same}",
           R.fmt(e))
-    return e
+    return q, r
 
 
 def _design(T, pv, N):

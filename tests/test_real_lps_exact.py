@@ -2,8 +2,9 @@
 long-horizon kernel, the storage-chain kernel and the band kernel, through check_exact -- objective, KKT residuals, x / y where
 unique, and on every LP the columns every optimum has at a bound and the reduced costs every optimal y zeroes.
 
-The launches are tiled as in test_stage_kernels_planted.py (2 x grid x problems_per_cta + 5 LPs, every copy bitwise equal to its
-first), and the same launch-geometry asserts show which kernel ran."""
+The launches are tiled as in test_stage_kernels_planted.py (2 x grid x problems_per_cta + 5 LPs in one launch, so that group
+slots and warps take second and third tickets; every copy bitwise equal to its first), and the same launch-geometry asserts show which
+kernel ran."""
 import numpy as np
 import pytest
 import torch
@@ -21,13 +22,23 @@ def _sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def _run(s, sol, name, N=None, cperm=None, rperm=None):
+def solve_device(sol, s, want_xy=True):
+    """set s in ONE launch through the device call, results as numpy.  The host call cuts a pageable batch into chunks of about
+    2 000 LPs, each its own launch, in which a group slot of a stage kernel rarely takes a second ticket."""
+    dev = torch.device("cuda")
+    r = sol.solve(torch.as_tensor(s.cparams, device=dev), torch.as_tensor(s.rparams, device=dev) if s.t.Pr else None,
+                  want_x=want_xy, want_y=want_xy)
+    torch.cuda.synchronize()
+    return S.LPResult(*(None if a is None else a.cpu().numpy() for a in (r.obj, r.status, r.iters, r.x, r.y)))
+
+
+def _run(s, sol, name, N=None, cperm=None, rperm=None, obj_rel=R.OBJ_REL):
     if N is None:
         big, _ = s.tile(40000)
-        sol.solve_host(big.cparams, big.rparams if s.t.Pr else None)
+        solve_device(sol, big, want_xy=False)
         N = 2 * S.last_launch()["grid"] * S.last_launch()["problems_per_cta"] + 5
     q, k = s.tile(N, seed=1)
-    r = sol.solve_host(q.cparams, q.rparams if s.t.Pr else None, want_x=True, want_y=True)
+    r = solve_device(sol, q)
     ll = S.last_launch()
     if name == "chain":
         # the chain kernel's own shared memory per warp and LPs per CTA (as in test_stage_kernels_planted._run)
@@ -48,7 +59,7 @@ def _run(s, sol, name, N=None, cperm=None, rperm=None):
     first = np.unique(k, return_index=True)[1]
     for a in (r.obj, r.status, r.iters, r.x, r.y):
         assert np.array_equal(a, a[first[k]])
-    e = R.check_exact(q, r.obj, r.status, r.x, r.y, cperm=cperm, rperm=rperm, kkt_rows=first, what=name)
+    e = R.check_exact(q, r.obj, r.status, r.x, r.y, cperm=cperm, rperm=rperm, kkt_rows=first, what=name, obj_rel=obj_rel)
     print(name, N, R.fmt(e))
     return q, r
 

@@ -2,8 +2,8 @@
 and the storage-chain kernel -- against exact optima (tests/planted_stage.py, tests/exact_lp.py): objective, x and y element by
 element in the caller's order, and the KKT residuals of every LP, at every geometry each family is instantiated for.
 
-Each case tiles a pool of certified LPs, in a random permutation, to 2 x grid x problems_per_cta + 5 LPs of a full launch: more
-than two waves of full CTAs, every LP group refilled and every slot reused.  Every copy of an LP must equal its first copy
+Each case tiles a pool of certified LPs, in a random permutation, to 2 x grid x problems_per_cta + 5 LPs of a full launch, solved in
+that one launch (test_real_lps_exact.solve_device): more than two waves of full CTAs, every LP group refilled and every slot reused.  Every copy of an LP must equal its first copy
 bitwise, so the KKT residuals are measured on the first copies only."""
 import functools
 
@@ -16,6 +16,7 @@ from dispatches_b200 import solver as S
 from planted_lp import shuffled
 from planted_stage import CHAIN_T, CHAIN_VARIANTS, chain_lanes, chain_smem_bytes, check, planted_chain, planted_wb
 from test_kernel_status_parity import _assert_kernel
+from test_real_lps_exact import solve_device
 
 pytestmark = pytest.mark.gpu
 
@@ -31,10 +32,10 @@ def _run(p, sol, name, N=None, t=None, cperm=None, rperm=None):
     of 40 000 LPs gives that geometry) -- and checks every LP against its exact optimum"""
     if N is None:
         big, _ = p.tile(40000)
-        sol.solve_host(big.cparams, big.rparams)
+        solve_device(sol, big, want_xy=False)
         N = 2 * S.last_launch()["grid"] * S.last_launch()["problems_per_cta"] + 5
     q, k = p.tile(N, seed=1)
-    r = sol.solve_host(q.cparams, q.rparams, want_x=True, want_y=True)
+    r = solve_device(sol, q)
     ll = S.last_launch()
     if name == "chain":
         # the chain kernel's own shared memory per warp, which no band-kernel placement matches (at L = 32 its problems_per_cta is
