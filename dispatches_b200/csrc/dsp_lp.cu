@@ -1116,6 +1116,24 @@ __global__ void __launch_bounds__(32 * kSensWarps) dsp_lp_sens_kernel(const sens
     }
 }
 
+}  // namespace
+
+#include "dsp_crossover.cuh"
+
+namespace {
+// crossover post-pass (dsp_crossover.cuh): persistent CTAs of kXoThreads threads, one LP per CTA, its work region (B^-1 and the LP's
+// vectors) in dynamic shared memory when it fits, else in the handle's workspace (ws_stride doubles per CTA)
+constexpr int kXoThreads = 256;
+static_assert(kXoThreads <= xo::kMaxThreads, "the crossover's reductions hold one entry per thread");
+__global__ void __launch_bounds__(kXoThreads) dsp_lp_crossover_kernel(const xo::Params P) {
+    extern __shared__ __align__(16) double xo_smem[];
+    __shared__ xo::Shared S;
+    double *w = P.ws ? P.ws + (long long)blockIdx.x * P.ws_stride : xo_smem;
+    const sens::View v = sens::view_of(P.blob, P.L);
+    const xo::View X = xo::view_of(P.xblob, P.X);
+    for (long long p = blockIdx.x; p < P.N; p += gridDim.x) xo::lp_body(P, v, X, w, &S, p, threadIdx.x, blockDim.x);
+}
+
 // FP64 FMA micro-benchmark: the measured denominator of the FP64 roofline fraction bench.py reports.  8 independent DFMA
 // chains per thread.
 __global__ void __launch_bounds__(256) dsp_fp64_peak_kernel(double *out, int iters, double a, double b) {
@@ -1195,7 +1213,7 @@ struct dsp_template {
         Csc At;
     } band;
     struct HostMaps {              // host copies of the parameter maps in internal order (umap: the first nb columns)
-        std::vector<double> c0, omap, ocmap, cm_val, bm_val, um_val;
+        std::vector<double> c0, b0, u0, omap, ocmap, cm_val, bm_val, um_val;
         std::vector<int> cm_ptr, cm_idx, bm_ptr, bm_idx, um_ptr, um_idx;
     } maps;
     struct Terms {                 // per-problem matrix terms in the caller's order: CSR position (internal order), rparams index, coef
@@ -1208,6 +1226,12 @@ struct dsp_template {
         sens::Layout L;
     };
     mutable Sens sns;
+    struct Xo {                    // the crossover's own structure blob (built at the first dsp_lp_crossover call)
+        bool ready;
+        const unsigned char *blob;
+        xo::Layout L;
+    };
+    mutable Xo xov;
     unsigned long long *ticket;
     // host-call staging (pinned) and device buffers, grown on demand
     int64_t cap_N;
@@ -1355,7 +1379,7 @@ int template_init(dsp_template *T, const dsp_template_desc *D) {
         upload(T, D->umap.val, D->umap.ptr[nb], &K.um_val))
         return DSP_E_CUDA;
     dsp_template::HostMaps &H = T->maps;
-    H.c0.assign(D->c0, D->c0 + n); H.omap.assign(D->omap, D->omap + D->Pr); H.ocmap.assign(D->ocmap, D->ocmap + D->Pc);
+    H.c0.assign(D->c0, D->c0 + n); H.b0.assign(D->b0, D->b0 + m); H.u0.assign(D->u0, D->u0 + nb); H.omap.assign(D->omap, D->omap + D->Pr); H.ocmap.assign(D->ocmap, D->ocmap + D->Pc);
     H.cm_ptr.assign(D->cmap.ptr, D->cmap.ptr + n + 1); H.cm_idx.assign(D->cmap.idx, D->cmap.idx + D->cmap.ptr[n]);
     H.cm_val.assign(D->cmap.val, D->cmap.val + D->cmap.ptr[n]);
     H.bm_ptr.assign(D->bmap.ptr, D->bmap.ptr + m + 1); H.bm_idx.assign(D->bmap.idx, D->bmap.idx + D->bmap.ptr[m]);
@@ -2158,6 +2182,72 @@ int dsp_lp_sensitivities(const dsp_template *T, int64_t N, const double *cparams
     return launched(blocks, 32 * kSensWarps, smem, kSensWarps);
 }
 
+// The crossover's structure: the sensitivity pass's blob (CSC of A0 with the matrix terms by entry, c0 and Cmap by column) and its
+// own (b0 and Bmap by row, u0 and Umap by column, the CSR of A with the CSC position of every entry), both in the caller's order
+static int ensure_xo(const dsp_template *T) {
+    if (int e = ensure_sens(T)) return e;
+    static std::mutex mu;
+    std::lock_guard<std::mutex> lk(mu);
+    if (T->xov.ready) return 0;
+    const KParams &K = T->kp;
+    const dsp_template::HostMaps &H = T->maps;
+    sens::HostTemplate S{K.m, K.n, K.nb, K.Pc, K.Pr, T->band.A_ptr, T->band.A_idx, T->band.A_val, T->col_perm, T->row_perm,
+                         H.c0, H.cm_ptr, H.cm_idx, H.cm_val, H.bm_ptr, H.bm_idx, H.bm_val, H.um_ptr, H.um_idx, H.um_val, H.omap, H.ocmap,
+                         T->mterms.q, T->mterms.param, T->mterms.coef};
+    std::vector<unsigned char> blob;
+    const xo::Layout L = xo::build_blob(S, H.b0, H.u0, blob);
+    dsp_template *Tm = const_cast<dsp_template *>(T);
+    if (int rc = upload(Tm, blob, &Tm->xov.blob)) return rc;
+    Tm->xov.L = L;
+    Tm->xov.ready = true;
+    return 0;
+}
+
+int dsp_lp_crossover(const dsp_template *T, int64_t N, const double *cparams, const double *rparams, int64_t rparams_stride,
+                     const int32_t *status, const double *x, const double *y, int32_t max_pivots, double *obj_out, double *x_out,
+                     double *y_out, int8_t *col_status, int8_t *row_basic, int32_t *xstatus, int32_t *pivots, void *cuda_stream) {
+    if (!T) { g_err = "dsp_lp_crossover: null handle"; return DSP_E_ARG; }
+    if (N < 0) { g_err = "dsp_lp_crossover: N < 0"; return DSP_E_ARG; }
+    if (T->kp.m > 1024) { g_err = "dsp_lp_crossover: crossover takes m <= 1024"; return DSP_E_ARG; }
+    if (N == 0) return 0;
+    if (!status || !x || !y) { g_err = "dsp_lp_crossover: status, x and y are required (solve with x and y)"; return DSP_E_ARG; }
+    if (!obj_out || !x_out || !y_out || !xstatus) { g_err = "dsp_lp_crossover: obj_out, x_out, y_out and xstatus are required"; return DSP_E_ARG; }
+    if (T->kp.Pc > 0 && !cparams) { g_err = "dsp_lp_crossover: cparams is NULL but the template has Pc > 0"; return DSP_E_ARG; }
+    if (T->kp.Pr > 0 && !rparams) { g_err = "dsp_lp_crossover: rparams is NULL but the template has Pr > 0"; return DSP_E_ARG; }
+    if (int e = ensure_xo(T)) return e;
+    const KParams &K = T->kp;
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    xo::Params P;
+    P.m = K.m; P.n = K.n; P.Pc = K.Pc; P.Pr = K.Pr; P.nnz = T->band.A_ptr[K.m];
+    P.N = N; P.cparams = cparams; P.rparams = rparams; P.rstride = rparams_stride;
+    P.status = status; P.x = x; P.y = y;
+    P.max_pivots = max_pivots > 0 ? max_pivots : DSP_CROSSOVER_DEFAULT_PIVOTS(K.m, K.n);
+    P.o0 = K.o0;
+    P.obj = obj_out; P.x_out = x_out; P.y_out = y_out; P.col_status = (signed char *)col_status; P.row_basic = (signed char *)row_basic;
+    P.xstatus = xstatus; P.pivots = pivots;
+    P.blob = T->sns.blob; P.L = T->sns.L; P.xblob = T->xov.blob; P.X = T->xov.L;
+    const long long wd = xo::work_doubles(K.m, K.n, P.nnz);
+    const size_t static_smem = sizeof(xo::Shared);
+    const bool in_smem = (size_t)wd * 8 + static_smem <= (size_t)T->smem_optin;
+    const size_t smem = in_smem ? (size_t)wd * 8 : 0;
+    if (int rc = allow_smem(dsp_lp_crossover_kernel, smem)) return rc;
+    int occ = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dsp_lp_crossover_kernel, kXoThreads, smem));
+    const long long resident = (long long)T->sm_count * std::max(occ, 1);
+    long long blocks;
+    if (in_smem) {
+        P.ws = nullptr; P.ws_stride = 0;
+        blocks = std::min<long long>(N, resident);
+    } else {
+        WsGrid g;
+        if (int rc = ws_grid(T, N, resident, 1, (size_t)wd * 8, st, &g)) return rc;
+        P.ws = T->ws; P.ws_stride = wd;
+        blocks = g.blocks;
+    }
+    dsp_lp_crossover_kernel<<<(unsigned)blocks, kXoThreads, smem, st>>>(P);
+    return launched(blocks, kXoThreads, smem, 1);
+}
+
 static void free_staging(dsp_template *T) {
     cudaFree(T->d_cp); cudaFree(T->d_rp); cudaFree(T->d_obj); cudaFree(T->d_x); cudaFree(T->d_y);
     cudaFree(T->d_status); cudaFree(T->d_iters);
@@ -2638,6 +2728,7 @@ int dsp_lp_template_set_matrix_params(dsp_template *T, int32_t count, const int3
     K.n_amap = count; K.amap_q = dq; K.amap_param = dp; K.amap_coef = dc; K.at_from = daf; K.asm_qa = dqa; K.asm_qb = dqb;
     T->mterms = {q, pr, cf};
     T->sns.ready = false;          // the sensitivity pass rebuilds its structure with these terms
+    T->xov.ready = false;          // and so does the crossover
     return 0;
 }
 

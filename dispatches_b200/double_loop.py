@@ -29,13 +29,28 @@ _FAMILIES = {"wind_battery": TP.wind_battery_operation, "nuclear": TP.nuclear_op
 
 
 def _lp_solve(mode, T, cparams, rparams, n_tracking_hour=1, options=None, family="wind_battery"):
-    """One batched solve of the operation template; returns (obj [N], status [N], columns {name: [N,T]})."""
-    key = (family, mode, T, n_tracking_hour, tuple(sorted((options or {}).items())))
+    """One batched solve of the operation template; returns (obj [N], status [N], columns {name: [N,T]}).  options["crossover"]:
+    the columns come from a vertex of each LP (BatchLPSolver.crossover), as a simplex solver such as the reference's CBC returns
+    them; an LP whose crossover does not end OPTIMAL keeps its interior-point solution."""
+    options = dict(options or {})
+    crossover = bool(options.pop("crossover", False))
+    key = (family, mode, T, n_tracking_hour, tuple(sorted(options.items())))
     if key not in _SOLVERS:
-        _SOLVERS[key] = BatchLPSolver(_FAMILIES[family](T, mode, n_tracking_hour), **(options or {}))
+        _SOLVERS[key] = BatchLPSolver(_FAMILIES[family](T, mode, n_tracking_hour), **options)
     sol = _SOLVERS[key]
-    r = sol.solve_host(np.ascontiguousarray(cparams), np.ascontiguousarray(rparams), want_x=True)
-    return r.obj, r.status, _columns(sol.t, sol.to_model_space(r.x), T)
+    if not crossover:
+        r = sol.solve_host(np.ascontiguousarray(cparams), np.ascontiguousarray(rparams), want_x=True)
+        return r.obj, r.status, _columns(sol.t, sol.to_model_space(r.x), T)
+    import torch
+    dev = torch.device("cuda", torch.cuda.current_device())
+    cp = torch.as_tensor(np.ascontiguousarray(cparams, float), device=dev)
+    rp = torch.as_tensor(np.ascontiguousarray(rparams, float), device=dev)
+    r = sol.solve(cp, rp, want_x=True, want_y=True)
+    v = sol.crossover(cp, rp, r)
+    ok = (v.status == OPTIMAL)
+    x = torch.where(ok[:, None], v.x, r.x).cpu().numpy()
+    obj = torch.where(ok, v.obj, r.obj).cpu().numpy()
+    return obj, r.status.cpu().numpy(), _columns(sol.t, sol.to_model_space(x), T)
 
 
 _COLS = dict(grid="blk[{t}].fs.splitter.grid_elec[0]", batt_in="blk[{t}].fs.battery.elec_in[0]",

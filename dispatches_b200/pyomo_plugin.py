@@ -112,7 +112,11 @@ class B200IPM:
     ``solve(model, tee=...)`` writing Var values (and ``model.dual`` / ``model.rc`` when the model declares an IMPORT Suffix of that
     name) back, returning SolverResults with solver.status / termination_condition.  ``options={"sensitivities": True}`` adds
     ``res.batch["d_params"]`` [N, P]: d objective / d every batched Param (a subgradient where the optimum is not unique), from the
-    GPU post-pass dsp_lp_sensitivities."""
+    GPU post-pass dsp_lp_sensitivities.  ``options={"crossover": True}`` (templates of up to 1024 rows) returns a vertex of every LP, as a
+simplex solver such as CBC does: a plain solve writes the vertex into the Vars, ``model.dual`` and ``model.rc`` (presolve's
+substitutions, splits and flips are affine bijections, so a vertex of the template is a vertex of the model); a batched solve returns
+the vertex in ``res.batch`` (``obj``, ``x``, ``duals``) with the basis and crossover status in ``res.batch["crossover"]``.  An LP
+whose crossover does not end OPTIMAL keeps its interior-point solution, and ``res.solver.message`` says so."""
 
     def __init__(self, **kw):
         self.options = dict(tol=1e-9, feas_tol=1e-9, max_iter=60)
@@ -141,15 +145,27 @@ class B200IPM:
         else:
             pv = p0[None, :] if p0.size else np.zeros((1, 0))
         sense = t.meta["sense"]
-        d_params = None
-        if opts.get("sensitivities"):
+        d_params = vertex = None
+        message = None
+        if opts.get("sensitivities") or opts.get("crossover"):
             # the device path: the same Param vector is cparams and rparams, so d obj / d Param = d_cparams + d_rparams
             import torch
             dev = torch.device("cuda", torch.cuda.current_device())
             pvt = torch.as_tensor(np.ascontiguousarray(pv, float), device=dev)
             rd = sol.solve(pvt, pvt if t.Pr else None, want_x=True, want_y=True)
-            g = sol.sensitivities(pvt, pvt if t.Pr else None, rd, want_rc=False)
-            d_params = sense * (g.d_cparams + g.d_rparams).cpu().numpy()
+            if opts.get("crossover"):
+                v = sol.crossover(pvt, pvt if t.Pr else None, rd)
+                ok = v.status == OPTIMAL
+                rd = LPResult(torch.where(ok, v.obj, rd.obj), rd.status, rd.iters, torch.where(ok[:, None], v.x, rd.x),
+                              torch.where(ok[:, None], v.y, rd.y))
+                vertex = {k: getattr(v, k).cpu().numpy() for k in ("status", "pivots", "col_status", "row_basic")}
+                lost = np.flatnonzero((vertex["status"] != OPTIMAL) & (rd.status.cpu().numpy() == OPTIMAL))
+                if lost.size:
+                    message = (f"crossover did not reach a vertex for {lost.size} LP(s) (first: {int(lost[0])}, crossover status "
+                               f"{int(vertex['status'][lost[0]])}): their interior-point solution is loaded")
+            if opts.get("sensitivities"):
+                g = sol.sensitivities(pvt, pvt if t.Pr else None, rd, want_rc=False)
+                d_params = sense * (g.d_cparams + g.d_rparams).cpu().numpy()
             r = LPResult(*(a.cpu().numpy() for a in (rd.obj, rd.status, rd.iters, rd.x, rd.y)))
         else:
             r = sol.solve_host(pv, pv if t.Pr else None, want_x=True, want_y=True)
@@ -177,6 +193,10 @@ class B200IPM:
         res.batch = dict(obj=sense * r.obj, status=r.status, iters=r.iters, x=xm, duals=ym, var_names=[v.name for v in vars_])
         if d_params is not None:
             res.batch["d_params"] = d_params
+        if vertex is not None:
+            res.batch["crossover"] = vertex
+        if message is not None:
+            res.solver.message = message
         if tee:
             print(f"b200ipm: {pv.shape[0]} LP(s), m={t.m} n={t.n} w={t.w}, iterations max {int(r.iters.max())}")
         return res

@@ -28,7 +28,7 @@ STATUS_NAMES = {OPTIMAL: "optimal", MAX_ITER: "maxIterations", NUMERICAL: "error
 KERNEL_AUTO, KERNEL_BAND, KERNEL_STAGE, KERNEL_STAGE_V1, KERNEL_DENSE, KERNEL_DENSE_CLUSTER, KERNEL_BAND_SPLIT = 0, 1, 2, 3, 4, 5, 6
 
 EXPORTS = ["dsp_lp_template_create", "dsp_lp_template_set_matrix_params", "dsp_lp_template_set_stage_chain1", "dsp_lp_template_create_csr", "dsp_lp_template_create_dense", "dsp_lp_template_create_dense_with_matrix_params", "dsp_lp_template_create_dense_cluster", "dsp_lp_analyze_csr", "dsp_lp_template_info", "dsp_lp_template_destroy", "dsp_lp_template_set_stage_wb", "dsp_lp_default_opts", "dsp_lp_solve_batch",
-           "dsp_lp_solve_batch_host", "dsp_lp_sensitivities", "dsp_lp_launch_count", "dsp_lp_last_launch", "dsp_lp_last_error",
+           "dsp_lp_solve_batch_host", "dsp_lp_sensitivities", "dsp_lp_crossover", "dsp_lp_launch_count", "dsp_lp_last_launch", "dsp_lp_last_error",
            "dsp_lp_version", "dsp_lp_fp64_peak_tflops"]
 
 
@@ -114,6 +114,9 @@ def load_library():
     lib.dsp_lp_solve_batch_host.restype = C.c_int
     lib.dsp_lp_sensitivities.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 7
     lib.dsp_lp_sensitivities.restype = C.c_int
+    lib.dsp_lp_crossover.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 3 + [C.c_int32] + \
+        [C.c_void_p] * 8
+    lib.dsp_lp_crossover.restype = C.c_int
     lib.dsp_lp_launch_count.restype = C.c_int64
     lib.dsp_lp_last_launch.argtypes = [C.POINTER(C.c_int32)] * 4
     lib.dsp_lp_last_launch.restype = C.c_int
@@ -155,6 +158,18 @@ class Sensitivities:
     rc: object           # [N,n] c - A'y, or None
     d_cparams: object    # [N,Pc]
     d_rparams: object    # [N,Pr]
+
+
+@dataclasses.dataclass
+class Vertex:
+    """dsp_lp_crossover (include/dsp_lp.h): a basic optimal solution of every LP a solve left OPTIMAL, in the caller's order"""
+    obj: object          # [N] c'x + k at the vertex
+    x: object            # [N,n] basic solution: every nonbasic column exactly at a bound
+    y: object            # [N,m] basis duals B^-T c_B
+    col_status: object   # [N,n] int8: 0 at 0, 1 basic, 2 at u (-1: LP not crossed over)
+    row_basic: object    # [N,m] int8: 1 where the row's artificial stays basic (a redundant row)
+    status: object       # [N] OPTIMAL / MAX_ITER / NUMERICAL, or the solve's status where that was not OPTIMAL
+    pivots: object       # [N] basis changes and bound flips after the crash
 
 
 def _i32(a):
@@ -355,6 +370,43 @@ class BatchLPSolver:
         rc = self.lib.dsp_lp_sensitivities(self.handle, N, ptr(cparams), rptr, rstride, result.status.data_ptr(), result.x.data_ptr(),
                                            result.y.data_ptr(), ptr(out.rc), ptr(out.d_cparams), ptr(out.d_rparams), C.c_void_p(stream))
         self._check(rc, "dsp_lp_sensitivities")
+        return out
+
+    def crossover(self, cparams, rparams, result, max_pivots=0):
+        """A vertex (basic optimal solution) of every OPTIMAL LP of a batch that ``solve`` returned with want_x = want_y = True for the
+        same cparams / rparams (CUDA tensors), m <= 1024.  max_pivots <= 0: the library's default.  One kernel launch on torch's
+        current stream, no synchronisation."""
+        import torch
+        t = self.t
+        if not torch.is_tensor(cparams) or not cparams.is_cuda or cparams.dtype != torch.float64 or cparams.dim() != 2 \
+                or cparams.shape[1] != t.Pc:
+            raise ValueError(f"cparams must be a CUDA float64 tensor of shape [N, {t.Pc}]")
+        N = cparams.shape[0]
+        dev = cparams.device
+        if result.x is None or result.y is None:
+            raise ValueError("the LPResult must carry x and y (solve with want_x=True, want_y=True)")
+        ok = lambda a, shape, dt: torch.is_tensor(a) and a.is_cuda and a.device == dev and a.is_contiguous() and tuple(a.shape) == shape \
+            and a.dtype == dt
+        if not (ok(result.status, (N,), torch.int32) and ok(result.x, (N, t.n), torch.float64) and ok(result.y, (N, t.m), torch.float64)):
+            raise ValueError(f"result.status / x / y must be contiguous CUDA [{N}] int32, [{N}, {t.n}] and [{N}, {t.m}] float64 tensors")
+        cparams = cparams.contiguous()
+        rstride, rptr = 0, None
+        if t.Pr:
+            if rparams is None or not torch.is_tensor(rparams) or not rparams.is_cuda or rparams.dtype != torch.float64 \
+                    or rparams.device != dev or tuple(rparams.shape) not in ((t.Pr,), (N, t.Pr)):
+                raise ValueError(f"rparams must be a CUDA float64 tensor of shape [{t.Pr}] or [{N}, {t.Pr}] on {dev}")
+            rparams = rparams.contiguous()
+            rstride = 0 if rparams.dim() == 1 else t.Pr
+            rptr = rparams.data_ptr()
+        e = lambda shape, dt: torch.empty(shape, dtype=dt, device=dev)
+        out = Vertex(e((N,), torch.float64), e((N, t.n), torch.float64), e((N, t.m), torch.float64), e((N, t.n), torch.int8),
+                     e((N, t.m), torch.int8), e((N,), torch.int32), e((N,), torch.int32))
+        ptr = lambda a: a.data_ptr() if a is not None and a.numel() else None
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.dsp_lp_crossover(self.handle, N, ptr(cparams), rptr, rstride, result.status.data_ptr(), result.x.data_ptr(),
+                                       result.y.data_ptr(), int(max_pivots), ptr(out.obj), ptr(out.x), ptr(out.y), ptr(out.col_status),
+                                       ptr(out.row_basic), ptr(out.status), ptr(out.pivots), C.c_void_p(stream))
+        self._check(rc, "dsp_lp_crossover")
         return out
 
     # ------------------------------------------------------------------ host arrays (copies included)

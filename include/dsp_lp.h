@@ -240,6 +240,39 @@ int dsp_lp_sensitivities(const dsp_template *t, int64_t N,
                          double *rc /*[N,n] or NULL*/, double *d_cparams /*[N,Pc] or NULL*/, double *d_rparams /*[N,Pr] or NULL*/,
                          void *cuda_stream);
 
+/* Crossover of a solved batch: for every LP whose status is DSP_OPTIMAL, a basic optimal solution (a vertex) of the same LP, from the
+ * (x, y) that dsp_lp_solve_batch returned for the same cparams / rparams.  An interior-point solve returns the analytic centre of the
+ * optimal face; a simplex solver (CBC, Gurobi, HiGHS) returns a vertex with basis duals, and this is that answer.  m <= 1024.
+ * The LP is  min c'x + k, A x = b, 0 <= x <= u  in the caller's column / row order, with every per-problem parameter and matrix term.
+ * A basis is col_status [n] (0: at 0, 1: basic, 2: at u) and row_basic [m] (1: the row's artificial column, a unit column with bounds
+ * [0, 0], is basic: a redundant row), m basic variables in all.  The outputs are that basis, its basic solution x_out (every nonbasic
+ * column exactly at its bound; a column with u = 0 is reported at the bound the sign of its reduced cost asks for), its duals
+ * y_out = B^-T c_B and obj_out = c'x + k.
+ * Algorithm (csrc/dsp_crossover.cuh, DESIGN.md 4.6): crash a basis from the most interior columns, push every other column inside its
+ * bounds onto a bound, then bounded primal / dual simplex pivots until the basis is primal and dual feasible within 1e-9 of the primal
+ * scale max(1, |b|_inf, |u_finite|_inf) and of |c|_inf, and every artificial a column can replace is pivoted out.  One CTA per LP
+ * with a dense explicit B^-1 (in shared memory up to m ~ 160, else about 8 m^2 bytes per CTA in flight of the handle's workspace).
+ * xstatus [N]: DSP_OPTIMAL (the final basic solution is primal and dual feasible within tolerance), DSP_MAX_ITER (max_pivots pivots;
+ * <= 0: DSP_CROSSOVER_DEFAULT_PIVOTS(m, n)), DSP_NUMERICAL (a singular reinversion, or a basis primal and dual infeasible at once);
+ * an LP whose input status is not DSP_OPTIMAL keeps that status and gets NaN in x_out / y_out / obj_out, -1 in col_status /
+ * row_basic and 0 pivots.  An LP that ends DSP_MAX_ITER or DSP_NUMERICAL gets the state the crossover stopped in: x_out / y_out /
+ * obj_out are finite but are not a basic optimal solution (x_out need not even be one of the LP's basic solutions), and col_status is
+ * -1 for a column the push had not yet moved onto a bound; callers should use the solve's own x / y for such LPs.
+ * pivots [N]: basis changes and bound flips after the crash.
+ * DEVICE pointers, stream-ordered, no synchronisation, the rparams_stride == 0 broadcast of dsp_lp_solve_batch.  Results are bitwise
+ * reproducible and do not depend on where an LP sits in the batch.  One kernel launch per call (none when N == 0); the first call on
+ * a handle builds its structure on the host.
+ * DSP_E_ARG: NULL handle, N < 0, m > 1024 ("crossover takes m <= 1024"), and for N > 0 NULL status / x / y / obj_out / x_out / y_out /
+ * xstatus, NULL cparams with Pc > 0 or NULL rparams with Pr > 0. */
+#define DSP_CROSSOVER_DEFAULT_PIVOTS(m, n) (10 * ((m) + (n)))
+int dsp_lp_crossover(const dsp_template *t, int64_t N,
+                     const double *cparams, const double *rparams, int64_t rparams_stride,
+                     const int32_t *status, const double *x, const double *y,
+                     int32_t max_pivots,
+                     double *obj_out /*[N]*/, double *x_out /*[N,n]*/, double *y_out /*[N,m]*/,
+                     int8_t *col_status /*[N,n] or NULL*/, int8_t *row_basic /*[N,m] or NULL*/,
+                     int32_t *xstatus /*[N]*/, int32_t *pivots /*[N] or NULL*/, void *cuda_stream);
+
 /* Introspection used by tests / bench: kernel launches issued so far, last launch geometry (grid in CTAs, block, dynamic shared
  * memory; problems_per_cta: LPs per CTA, or for the dense cluster kernel the cluster size in CTAs). */
 int64_t dsp_lp_launch_count(void);
