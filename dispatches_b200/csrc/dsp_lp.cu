@@ -1134,6 +1134,22 @@ __global__ void __launch_bounds__(kXoThreads) dsp_lp_crossover_kernel(const xo::
     for (long long p = blockIdx.x; p < P.N; p += gridDim.x) xo::lp_body(P, v, X, w, &S, p, threadIdx.x, blockDim.x);
 }
 
+}  // namespace
+
+#include "dsp_ranging.cuh"
+
+namespace {
+// ranging post-pass (dsp_ranging.cuh): the crossover's geometry, one LP per CTA, its work region in dynamic shared memory when it fits,
+// else in the handle's workspace
+__global__ void __launch_bounds__(kXoThreads) dsp_lp_ranging_kernel(const rg::Params P) {
+    extern __shared__ __align__(16) double rg_smem[];
+    __shared__ xo::Shared S;
+    double *w = P.ws ? P.ws + (long long)blockIdx.x * P.ws_stride : rg_smem;
+    const sens::View v = sens::view_of(P.blob, P.L);
+    const xo::View X = xo::view_of(P.xblob, P.X);
+    for (long long p = blockIdx.x; p < P.N; p += gridDim.x) rg::lp_body(P, v, X, w, &S, p, threadIdx.x, blockDim.x);
+}
+
 // FP64 FMA micro-benchmark: the measured denominator of the FP64 roofline fraction bench.py reports.  8 independent DFMA
 // chains per thread.
 __global__ void __launch_bounds__(256) dsp_fp64_peak_kernel(double *out, int iters, double a, double b) {
@@ -2203,6 +2219,29 @@ static int ensure_xo(const dsp_template *T) {
     return 0;
 }
 
+// The placement of a one-LP-per-CTA post-pass (crossover, ranging) whose LP has a work region of wd doubles: dynamic shared memory when
+// it fits beside xo::Shared, with as many CTAs as are resident; else the handle's workspace, ws_stride doubles per CTA
+struct XoGrid { long long blocks; size_t smem; double *ws; long long ws_stride; };
+extern "C++" template <class Kernel>
+int xo_grid(const dsp_template *T, Kernel kernel, long long N, long long wd, cudaStream_t st, XoGrid *out) {
+    const bool in_smem = (size_t)wd * 8 + sizeof(xo::Shared) <= (size_t)T->smem_optin;
+    out->smem = in_smem ? (size_t)wd * 8 : 0;
+    if (int rc = allow_smem(kernel, out->smem)) return rc;
+    int occ = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kXoThreads, out->smem));
+    const long long resident = (long long)T->sm_count * std::max(occ, 1);
+    if (in_smem) {
+        out->ws = nullptr; out->ws_stride = 0;
+        out->blocks = std::min<long long>(N, resident);
+    } else {
+        WsGrid g;
+        if (int rc = ws_grid(T, N, resident, 1, (size_t)wd * 8, st, &g)) return rc;
+        out->ws = T->ws; out->ws_stride = wd;
+        out->blocks = g.blocks;
+    }
+    return 0;
+}
+
 int dsp_lp_crossover(const dsp_template *T, int64_t N, const double *cparams, const double *rparams, int64_t rparams_stride,
                      const int32_t *status, const double *x, const double *y, int32_t max_pivots, double *obj_out, double *x_out,
                      double *y_out, int8_t *col_status, int8_t *row_basic, int32_t *xstatus, int32_t *pivots, void *cuda_stream) {
@@ -2226,26 +2265,42 @@ int dsp_lp_crossover(const dsp_template *T, int64_t N, const double *cparams, co
     P.obj = obj_out; P.x_out = x_out; P.y_out = y_out; P.col_status = (signed char *)col_status; P.row_basic = (signed char *)row_basic;
     P.xstatus = xstatus; P.pivots = pivots;
     P.blob = T->sns.blob; P.L = T->sns.L; P.xblob = T->xov.blob; P.X = T->xov.L;
-    const long long wd = xo::work_doubles(K.m, K.n, P.nnz);
-    const size_t static_smem = sizeof(xo::Shared);
-    const bool in_smem = (size_t)wd * 8 + static_smem <= (size_t)T->smem_optin;
-    const size_t smem = in_smem ? (size_t)wd * 8 : 0;
-    if (int rc = allow_smem(dsp_lp_crossover_kernel, smem)) return rc;
-    int occ = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, dsp_lp_crossover_kernel, kXoThreads, smem));
-    const long long resident = (long long)T->sm_count * std::max(occ, 1);
-    long long blocks;
-    if (in_smem) {
-        P.ws = nullptr; P.ws_stride = 0;
-        blocks = std::min<long long>(N, resident);
-    } else {
-        WsGrid g;
-        if (int rc = ws_grid(T, N, resident, 1, (size_t)wd * 8, st, &g)) return rc;
-        P.ws = T->ws; P.ws_stride = wd;
-        blocks = g.blocks;
-    }
-    dsp_lp_crossover_kernel<<<(unsigned)blocks, kXoThreads, smem, st>>>(P);
-    return launched(blocks, kXoThreads, smem, 1);
+    XoGrid g;
+    if (int rc = xo_grid(T, dsp_lp_crossover_kernel, N, xo::work_doubles(K.m, K.n, P.nnz), st, &g)) return rc;
+    P.ws = g.ws; P.ws_stride = g.ws_stride;
+    dsp_lp_crossover_kernel<<<(unsigned)g.blocks, kXoThreads, g.smem, st>>>(P);
+    return launched(g.blocks, kXoThreads, g.smem, 1);
+}
+
+int dsp_lp_ranging(const dsp_template *T, int64_t N, const double *cparams, const double *rparams, int64_t rparams_stride,
+                   const int32_t *xstatus, const int8_t *col_status, const int8_t *row_basic, int32_t Kd, const double *dir_c,
+                   const double *dir_r, int64_t dir_stride, double *theta_lo, double *theta_hi, double *dobj, double *d2obj,
+                   int32_t *rstatus, void *cuda_stream) {
+    if (!T) { g_err = "dsp_lp_ranging: null handle"; return DSP_E_ARG; }
+    if (N < 0) { g_err = "dsp_lp_ranging: N < 0"; return DSP_E_ARG; }
+    if (Kd < 0) { g_err = "dsp_lp_ranging: K < 0"; return DSP_E_ARG; }
+    if (T->kp.m > 1024) { g_err = "dsp_lp_ranging: ranging takes m <= 1024"; return DSP_E_ARG; }
+    if (N == 0 || Kd == 0) return 0;
+    if (!xstatus || !col_status || !row_basic) { g_err = "dsp_lp_ranging: xstatus, col_status and row_basic are required"; return DSP_E_ARG; }
+    if (!theta_lo || !theta_hi || !rstatus) { g_err = "dsp_lp_ranging: theta_lo, theta_hi and rstatus are required"; return DSP_E_ARG; }
+    if (T->kp.Pc > 0 && !cparams) { g_err = "dsp_lp_ranging: cparams is NULL but the template has Pc > 0"; return DSP_E_ARG; }
+    if (T->kp.Pr > 0 && !rparams) { g_err = "dsp_lp_ranging: rparams is NULL but the template has Pr > 0"; return DSP_E_ARG; }
+    if (int e = ensure_xo(T)) return e;
+    const KParams &K = T->kp;
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    rg::Params P;
+    P.m = K.m; P.n = K.n; P.Pc = K.Pc; P.Pr = K.Pr; P.nnz = T->band.A_ptr[K.m]; P.K = Kd;
+    P.N = N; P.cparams = cparams; P.rparams = rparams; P.rstride = rparams_stride;
+    P.status = xstatus; P.col_status = (const signed char *)col_status; P.row_basic = (const signed char *)row_basic;
+    P.dir_c = K.Pc > 0 ? dir_c : nullptr; P.dir_r = K.Pr > 0 ? dir_r : nullptr; P.dir_per_lp = dir_stride != 0;
+    P.o0 = K.o0;
+    P.lo = theta_lo; P.hi = theta_hi; P.dobj = dobj; P.d2obj = d2obj; P.rstatus = rstatus;
+    P.blob = T->sns.blob; P.L = T->sns.L; P.xblob = T->xov.blob; P.X = T->xov.L;
+    XoGrid g;
+    if (int rc = xo_grid(T, dsp_lp_ranging_kernel, N, rg::work_doubles(K.m, K.n, P.nnz), st, &g)) return rc;
+    P.ws = g.ws; P.ws_stride = g.ws_stride;
+    dsp_lp_ranging_kernel<<<(unsigned)g.blocks, kXoThreads, g.smem, st>>>(P);
+    return launched(g.blocks, kXoThreads, g.smem, 1);
 }
 
 static void free_staging(dsp_template *T) {

@@ -65,6 +65,11 @@ class PriceTakerResult:
     marginal_npv: dict | None = None
     # want_sensitivities=True (nuclear case, whose objective is an operating cost, not -1e-5 NPV): d obj / d LMP [N,T] under "lmp"
     marginal_obj: dict | None = None
+    # want_ranges=True: absolute [lo, hi] intervals of each parameter, all others fixed, over which the returned schedule (a vertex)
+    # stays optimal (include/dsp_lp.h: dsp_lp_ranging): "lmp" [N,T,2] in $/MWh; "wind_mw", "batt_mw", "pem_mw" [N,2] in MW and
+    # "h2_price_per_kg" [N,2] where the case has them.  Inside an interval the objective is linear in that parameter.  NaN rows for
+    # an LP whose crossover did not end OPTIMAL (it keeps its interior-point solution).
+    ranges: dict | None = None
 
     @property
     def NPV(self):
@@ -123,16 +128,63 @@ def _lmps(input_params, T):
     return np.ascontiguousarray(lmp)
 
 
-def _solve_with_sensitivities(sol, cp, rp):
-    """the batch through the device path (dsp_lp_solve_batch with x and y, then dsp_lp_sensitivities) on cuda:0; numpy results"""
+def _solve_on_device(sol, cp, rp, want_sensitivities=False, directions=None):
+    """the batch through the device path on cuda:0 (dsp_lp_solve_batch with x and y); with directions (dir_c [N,K,Pc], dir_r [N,K,Pr]
+    or None) also dsp_lp_crossover, whose vertex replaces the interior point of every LP it takes OPTIMAL, and dsp_lp_ranging of that
+    basis; with want_sensitivities dsp_lp_sensitivities at the returned (x, y).  numpy results: (LPResult, d_cparams, d_rparams,
+    theta_lo, theta_hi), None where not asked for"""
     import torch
     dev = torch.device("cuda", 0)
     cpt = torch.as_tensor(np.ascontiguousarray(cp, float), device=dev)
     rpt = torch.as_tensor(np.ascontiguousarray(rp, float), device=dev) if rp is not None else None
-    r = sol.solve(cpt, rpt, want_x=True, want_y=True)
-    g = sol.sensitivities(cpt, rpt, r, want_rc=False)
     host = lambda a: a.cpu().numpy()
-    return LPResult(host(r.obj), host(r.status), host(r.iters), host(r.x), host(r.y)), host(g.d_cparams), host(g.d_rparams)
+    r = sol.solve(cpt, rpt, want_x=True, want_y=True)
+    lo = hi = dc = dr = None
+    if directions is not None:
+        v = sol.crossover(cpt, rpt, r)
+        ok = v.status == OPTIMAL
+        r = LPResult(torch.where(ok, v.obj, r.obj), r.status, r.iters, torch.where(ok[:, None], v.x, r.x), torch.where(ok[:, None], v.y, r.y))
+        gc, gr = (None if d is None else torch.as_tensor(np.ascontiguousarray(d, float), device=dev) for d in directions)
+        g = sol.ranging(cpt, rpt, v, gc, gr)
+        lo, hi = host(g.theta_lo), host(g.theta_hi)
+    if want_sensitivities:
+        g = sol.sensitivities(cpt, rpt, r, want_rc=False)
+        dc, dr = host(g.d_cparams), host(g.d_rparams)
+    return LPResult(host(r.obj), host(r.status), host(r.iters), host(r.x), host(r.y)), dc, dr, lo, hi
+
+
+def _wind_directions(T, cf, N, pem=False):
+    """directions of wind_battery(_pem)'s parameters per LP, one per LMP hour (1 $/MWh)(, the hydrogen price: 1 $/kg), then wind,
+    battery(, PEM) sizes (1 MW: wind moves wind_kw cf_t and wind_kw, so its direction has the LP's own cf_t) -> (dir_c, dir_r)"""
+    cf = np.broadcast_to(np.asarray(cf, float), (N, T))
+    Pc, Pr = T + pem, T + 2 + pem
+    K = Pc + 2 + pem
+    dc, dr = np.zeros((N, K, Pc)), np.zeros((N, K, Pr))
+    dc[:, :Pc, :] = np.eye(Pc)
+    dr[:, Pc, :T] = 1e3 * cf
+    dr[:, Pc, T + 1] = 1e3
+    dr[:, Pc + 1, T] = 1e3
+    if pem:
+        dr[:, Pc + 2, T + 2] = 1e3
+    return dc, dr
+
+
+def _absolute(values, lo, hi):
+    """[..., 2] intervals values + [theta_lo, theta_hi]"""
+    return np.stack([values + lo, values + hi], axis=-1)
+
+
+def _wind_ranges(T, lmp, input_params, lo, hi, h2=None):
+    """PriceTakerResult.ranges of wind_battery(_pem) from the ranging along _wind_directions"""
+    N = lmp.shape[0]
+    size = lambda key: np.broadcast_to(np.asarray(input_params[key], float), (N,))
+    pem = h2 is not None
+    Pc = T + pem
+    out = dict(lmp=_absolute(lmp, lo[:, :T], hi[:, :T]), wind_mw=_absolute(size("wind_mw"), lo[:, Pc], hi[:, Pc]),
+               batt_mw=_absolute(size("batt_mw"), lo[:, Pc + 1], hi[:, Pc + 1]))
+    if pem:
+        out.update(h2_price_per_kg=_absolute(h2, lo[:, T], hi[:, T]), pem_mw=_absolute(size("pem_mw"), lo[:, Pc + 2], hi[:, Pc + 2]))
+    return out
 
 
 def _wind_marginals(T, cf, dc, dr, N, pem=False):
@@ -144,14 +196,19 @@ def _wind_marginals(T, cf, dc, dr, N, pem=False):
     return out
 
 
-def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solution=True, kernel=None, want_sensitivities=False):
+def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solution=True, kernel=None, want_sensitivities=False,
+                          want_ranges=False):
     """kernel: a solver.KERNEL_* choice for the band-template paths (None: the library's default, e.g. KERNEL_BAND_SPLIT for a long
     horizon on the split band kernel); the free-wind design (per-problem matrix coefficients) does not take it.
-    want_sensitivities (fixed design only): fill PriceTakerResult.marginal_npv (wind_mw, batt_mw, lmp)."""
+    want_sensitivities (fixed design only): fill PriceTakerResult.marginal_npv (wind_mw, batt_mw, lmp).
+    want_ranges (fixed design only, templates of up to 1024 rows): solve, cross over to a vertex and fill PriceTakerResult.ranges
+    (lmp, wind_mw, batt_mw); the returned schedule is the vertex (and marginal_npv, when asked for, its gradient)."""
     T = int(n_time_points)
     design = bool(input_params.get("design_opt", False))
     if want_sensitivities and design:
         raise NotImplementedError("want_sensitivities needs a fixed design (design_opt=False)")
+    if want_ranges and design:
+        raise NotImplementedError("want_ranges needs a fixed design (design_opt=False)")
     lmp = _lmps(input_params, T)
     cf = _capacity_factors(input_params, T)
     if design and not input_params.get("extant_wind", True):
@@ -164,10 +221,14 @@ def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solut
         rp = rp[0]
     elif rp.shape[0] != lmp.shape[0]:
         raise ValueError("sizes / capacity factors must be scalar or match the number of LMP scenarios")
-    marginal = None
-    if want_sensitivities:
-        r, dc, dr = _solve_with_sensitivities(sol, lmp, rp)
-        marginal = _wind_marginals(T, cf, dc, dr, lmp.shape[0])
+    marginal = ranges = None
+    if want_sensitivities or want_ranges:
+        dirs = _wind_directions(T, cf, lmp.shape[0]) if want_ranges else None
+        r, dc, dr, lo, hi = _solve_on_device(sol, lmp, rp, want_sensitivities, dirs)
+        if want_sensitivities:
+            marginal = _wind_marginals(T, cf, dc, dr, lmp.shape[0])
+        if want_ranges:
+            ranges = _wind_ranges(T, lmp, input_params, lo, hi)
     else:
         r = sol.solve_host(lmp, rp, want_x=want_solution)
     if verbose:
@@ -179,7 +240,7 @@ def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solut
     xm = sol.to_model_space(r.x) if want_solution else None
     if design:                                        # optimised size: value(m.battery_system_capacity)
         sizes["batt_kw"] = xm[:, sol.t.col_names.index("blk[0].fs.battery.nameplate_power")].copy()
-    return PriceTakerResult("wind_battery", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes, marginal)
+    return PriceTakerResult("wind_battery", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes, marginal, ranges=ranges)
 
 
 def _wind_battery_free_wind(T, lmp, cf, input_params, verbose):
@@ -216,12 +277,17 @@ def _wind_battery_free_wind(T, lmp, cf, input_params, verbose):
     return PriceTakerResult("wind_battery", T, lmp, r.obj, r.status, r.iters, xm, names, sizes)
 
 
-def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_solution=True, kernel=None, want_sensitivities=False):
+def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_solution=True, kernel=None, want_sensitivities=False,
+                              want_ranges=False):
     """kernel: a solver.KERNEL_* choice (None: the library's default).  want_sensitivities (fixed design only): fill
-    PriceTakerResult.marginal_npv (wind_mw, batt_mw, pem_mw, h2_price_per_kg, lmp)."""
+    PriceTakerResult.marginal_npv (wind_mw, batt_mw, pem_mw, h2_price_per_kg, lmp).  want_ranges (fixed design only, templates of
+    up to 1024 rows): solve, cross over to a vertex and fill PriceTakerResult.ranges (lmp, wind_mw, batt_mw, pem_mw,
+    h2_price_per_kg); the returned schedule is the vertex (and marginal_npv, when asked for, its gradient)."""
     mode = input_params.get("design_opt", False)
     if want_sensitivities and mode is not False:
         raise NotImplementedError("want_sensitivities needs a fixed design (design_opt=False)")
+    if want_ranges and mode is not False:
+        raise NotImplementedError("want_ranges needs a fixed design (design_opt=False)")
     if mode not in (False, "PEM") or (mode == "PEM" and not input_params.get("extant_wind", True)):
         raise NotImplementedError("only design_opt False and \"PEM\" (extant wind) are on the batched GPU path")
     pem_design = mode == "PEM"
@@ -230,9 +296,9 @@ def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_sol
     N = lmp.shape[0]
     cf = _capacity_factors(input_params, T)
     batt = np.zeros(1) if pem_design else np.asarray(input_params["batt_mw"], float)   # "PEM" fixes the battery at 0 (:228)
-    # without a battery the template drops its columns; the sensitivities keep them (bounded by a zero size through Umap), so that
-    # d NPV / d batt_mw at 0 is the value of the first MW of battery, not only its cost
-    with_batt = bool(np.any(batt > 0)) or want_sensitivities
+    # without a battery the template drops its columns; the sensitivities and ranges keep them (bounded by a zero size through Umap),
+    # so that d NPV / d batt_mw at 0 is the value of the first MW of battery, not only its cost, and batt_mw has a range
+    with_batt = bool(np.any(batt > 0)) or want_sensitivities or want_ranges
     want_solution = want_solution or pem_design
     sol = get_solver("wind_battery_pem", T, kernel=kernel, with_battery=with_batt, extant_wind=bool(input_params.get("extant_wind", True)),
                      pem_design=pem_design)
@@ -243,10 +309,14 @@ def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_sol
         raise ValueError("sizes / capacity factors must be scalar or match the number of LMP scenarios")
     h2 = np.broadcast_to(np.asarray(input_params["h2_price_per_kg"], float), (N,))
     cp = np.ascontiguousarray(np.concatenate([lmp, h2[:, None]], axis=1))
-    marginal = None
-    if want_sensitivities:
-        r, dc, dr = _solve_with_sensitivities(sol, cp, rp)
-        marginal = _wind_marginals(T, cf, dc, dr, N, pem=True)
+    marginal = ranges = None
+    if want_sensitivities or want_ranges:
+        dirs = _wind_directions(T, cf, N, pem=True) if want_ranges else None
+        r, dc, dr, lo, hi = _solve_on_device(sol, cp, rp, want_sensitivities, dirs)
+        if want_sensitivities:
+            marginal = _wind_marginals(T, cf, dc, dr, N, pem=True)
+        if want_ranges:
+            ranges = _wind_ranges(T, lmp, dict(input_params, batt_mw=batt), lo, hi, h2=h2)
     else:
         r = sol.solve_host(cp, rp, want_x=want_solution)
     sizes = dict(wind_kw=np.broadcast_to(np.asarray(input_params["wind_mw"], float) * 1e3, (N,)),
@@ -255,23 +325,32 @@ def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_sol
     xm = sol.to_model_space(r.x) if want_solution else None
     if pem_design:                                    # optimised size: value(m.pem_system_capacity)
         sizes["pem_kw"] = xm[:, sol.t.col_names.index("pem_system_capacity[0]")].copy()
-    return PriceTakerResult("wind_battery_pem", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes, marginal)
+    return PriceTakerResult("wind_battery_pem", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes, marginal, ranges=ranges)
 
 
-def nuclear_dispatch_optimize(n_time_points, lmps, want_solution=False, kernel=None, want_sensitivities=False, **flowsheet_options):
+def nuclear_dispatch_optimize(n_time_points, lmps, want_solution=False, kernel=None, want_sensitivities=False, want_ranges=False,
+                              **flowsheet_options):
     """kernel: a solver.KERNEL_* choice (None: the library's default).  want_sensitivities: fill PriceTakerResult.marginal_obj["lmp"]
-    = d obj / d lmp [N,T] (the sizes are template constants, not parameters)."""
+    = d obj / d lmp [N,T] (the sizes are template constants, not parameters).  want_ranges (templates of up to 1024 rows): solve,
+    cross over to a vertex and fill PriceTakerResult.ranges["lmp"]; the returned schedule is the vertex (and marginal_obj, when asked
+    for, its gradient)."""
     T = int(n_time_points)
     lmp = np.ascontiguousarray(np.atleast_2d(np.asarray(lmps, float))[:, :T])
     sol = get_solver("nuclear", T, kernel=kernel, **flowsheet_options)
-    marginal = None
-    if want_sensitivities:
-        r, dc, _ = _solve_with_sensitivities(sol, lmp, None)
-        marginal = dict(lmp=dc[:, :T])
+    marginal = ranges = None
+    if want_sensitivities or want_ranges:
+        N, Pc = lmp.shape[0], sol.t.Pc
+        dirs = (np.broadcast_to(np.eye(T, Pc), (N, T, Pc)), None) if want_ranges else None
+        r, dc, _, lo, hi = _solve_on_device(sol, lmp, None, want_sensitivities, dirs)
+        if want_sensitivities:
+            marginal = dict(lmp=dc[:, :T])
+        if want_ranges:
+            ranges = dict(lmp=_absolute(lmp, lo, hi))
     else:
         r = sol.solve_host(lmp, None, want_x=want_solution)
     return PriceTakerResult("nuclear", T, lmp, r.obj, r.status, r.iters,
-                            sol.to_model_space(r.x) if want_solution else None, sol.t.col_names, {}, marginal_obj=marginal)
+                            sol.to_model_space(r.x) if want_solution else None, sol.t.col_names, {}, marginal_obj=marginal,
+                            ranges=ranges)
 
 
 _SOLAR_COST_KEYS = ("pv_cap_cost", "pv_op_cost", "batt_cap_cost_kw", "batt_cap_cost_kwh", "pem_cap_cost", "pem_op_cost", "pem_var_cost",

@@ -116,7 +116,10 @@ class B200IPM:
 simplex solver such as CBC does: a plain solve writes the vertex into the Vars, ``model.dual`` and ``model.rc`` (presolve's
 substitutions, splits and flips are affine bijections, so a vertex of the template is a vertex of the model); a batched solve returns
 the vertex in ``res.batch`` (``obj``, ``x``, ``duals``) with the basis and crossover status in ``res.batch["crossover"]``.  An LP
-whose crossover does not end OPTIMAL keeps its interior-point solution, and ``res.solver.message`` says so."""
+whose crossover does not end OPTIMAL keeps its interior-point solution, and ``res.solver.message`` says so.
+``options={"ranging": True}`` implies crossover and adds ``res.batch["param_ranges"]`` [N, P, 2]: for every batched Param, all others
+fixed, the absolute [lo, hi] values over which the LP's vertex stays optimal (GPU post-pass dsp_lp_ranging along the Param's axis; NaN
+for an LP whose crossover did not end OPTIMAL and for a Param that is a coefficient of the constraint matrix)."""
 
     def __init__(self, **kw):
         self.options = dict(tol=1e-9, feas_tol=1e-9, max_iter=60)
@@ -145,15 +148,15 @@ whose crossover does not end OPTIMAL keeps its interior-point solution, and ``re
         else:
             pv = p0[None, :] if p0.size else np.zeros((1, 0))
         sense = t.meta["sense"]
-        d_params = vertex = None
+        d_params = vertex = param_ranges = None
         message = None
-        if opts.get("sensitivities") or opts.get("crossover"):
+        if opts.get("sensitivities") or opts.get("crossover") or opts.get("ranging"):
             # the device path: the same Param vector is cparams and rparams, so d obj / d Param = d_cparams + d_rparams
             import torch
             dev = torch.device("cuda", torch.cuda.current_device())
             pvt = torch.as_tensor(np.ascontiguousarray(pv, float), device=dev)
             rd = sol.solve(pvt, pvt if t.Pr else None, want_x=True, want_y=True)
-            if opts.get("crossover"):
+            if opts.get("crossover") or opts.get("ranging"):
                 v = sol.crossover(pvt, pvt if t.Pr else None, rd)
                 ok = v.status == OPTIMAL
                 rd = LPResult(torch.where(ok, v.obj, rd.obj), rd.status, rd.iters, torch.where(ok[:, None], v.x, rd.x),
@@ -163,6 +166,15 @@ whose crossover does not end OPTIMAL keeps its interior-point solution, and ``re
                 if lost.size:
                     message = (f"crossover did not reach a vertex for {lost.size} LP(s) (first: {int(lost[0])}, crossover status "
                                f"{int(vertex['status'][lost[0]])}): their interior-point solution is loaded")
+            if opts.get("ranging"):
+                # Param k moves its cparams and its rparams entry together: the direction (e_k, e_k)
+                P = pv.shape[1]
+                lo = hi = np.zeros((pv.shape[0], 0))
+                if P:
+                    eye = torch.eye(P, dtype=torch.float64, device=dev)
+                    g = sol.ranging(pvt, pvt if t.Pr else None, v, eye, eye if t.Pr else None)
+                    lo, hi = g.theta_lo.cpu().numpy(), g.theta_hi.cpu().numpy()
+                param_ranges = np.stack([pv + lo, pv + hi], axis=-1)
             if opts.get("sensitivities"):
                 g = sol.sensitivities(pvt, pvt if t.Pr else None, rd, want_rc=False)
                 d_params = sense * (g.d_cparams + g.d_rparams).cpu().numpy()
@@ -195,6 +207,8 @@ whose crossover does not end OPTIMAL keeps its interior-point solution, and ``re
             res.batch["d_params"] = d_params
         if vertex is not None:
             res.batch["crossover"] = vertex
+        if param_ranges is not None:
+            res.batch["param_ranges"] = param_ranges
         if message is not None:
             res.solver.message = message
         if tee:

@@ -28,7 +28,7 @@ STATUS_NAMES = {OPTIMAL: "optimal", MAX_ITER: "maxIterations", NUMERICAL: "error
 KERNEL_AUTO, KERNEL_BAND, KERNEL_STAGE, KERNEL_STAGE_V1, KERNEL_DENSE, KERNEL_DENSE_CLUSTER, KERNEL_BAND_SPLIT = 0, 1, 2, 3, 4, 5, 6
 
 EXPORTS = ["dsp_lp_template_create", "dsp_lp_template_set_matrix_params", "dsp_lp_template_set_stage_chain1", "dsp_lp_template_create_csr", "dsp_lp_template_create_dense", "dsp_lp_template_create_dense_with_matrix_params", "dsp_lp_template_create_dense_cluster", "dsp_lp_analyze_csr", "dsp_lp_template_info", "dsp_lp_template_destroy", "dsp_lp_template_set_stage_wb", "dsp_lp_default_opts", "dsp_lp_solve_batch",
-           "dsp_lp_solve_batch_host", "dsp_lp_sensitivities", "dsp_lp_crossover", "dsp_lp_launch_count", "dsp_lp_last_launch", "dsp_lp_last_error",
+           "dsp_lp_solve_batch_host", "dsp_lp_sensitivities", "dsp_lp_crossover", "dsp_lp_ranging", "dsp_lp_launch_count", "dsp_lp_last_launch", "dsp_lp_last_error",
            "dsp_lp_version", "dsp_lp_fp64_peak_tflops"]
 
 
@@ -117,6 +117,9 @@ def load_library():
     lib.dsp_lp_crossover.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 3 + [C.c_int32] + \
         [C.c_void_p] * 8
     lib.dsp_lp_crossover.restype = C.c_int
+    lib.dsp_lp_ranging.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 3 + [C.c_int32] + \
+        [C.c_void_p] * 2 + [C.c_int64] + [C.c_void_p] * 6
+    lib.dsp_lp_ranging.restype = C.c_int
     lib.dsp_lp_launch_count.restype = C.c_int64
     lib.dsp_lp_last_launch.argtypes = [C.POINTER(C.c_int32)] * 4
     lib.dsp_lp_last_launch.restype = C.c_int
@@ -170,6 +173,16 @@ class Vertex:
     row_basic: object    # [N,m] int8: 1 where the row's artificial stays basic (a redundant row)
     status: object       # [N] OPTIMAL / MAX_ITER / NUMERICAL, or the solve's status where that was not OPTIMAL
     pivots: object       # [N] basis changes and bound flips after the crash
+
+
+@dataclasses.dataclass
+class Ranges:
+    """dsp_lp_ranging (include/dsp_lp.h): along every direction k, the theta interval over which an LP's basis stays optimal"""
+    theta_lo: object     # [N,K] <= 0 (-inf: unbounded); NaN where the LP is not OPTIMAL or the direction moves A
+    theta_hi: object     # [N,K] >= 0 (+inf: unbounded)
+    dobj: object         # [N,K] obj(theta) = obj + dobj theta + d2obj theta^2 / 2 inside the range
+    d2obj: object        # [N,K]
+    status: object       # [N] OPTIMAL / NUMERICAL, or the basis' status where that was not OPTIMAL
 
 
 def _i32(a):
@@ -370,6 +383,61 @@ class BatchLPSolver:
         rc = self.lib.dsp_lp_sensitivities(self.handle, N, ptr(cparams), rptr, rstride, result.status.data_ptr(), result.x.data_ptr(),
                                            result.y.data_ptr(), ptr(out.rc), ptr(out.d_cparams), ptr(out.d_rparams), C.c_void_p(stream))
         self._check(rc, "dsp_lp_sensitivities")
+        return out
+
+    def ranging(self, cparams, rparams, vertex, dir_c=None, dir_r=None):
+        """Ranges of the bases of a ``crossover`` result (a Vertex, or any object with status, col_status and row_basic CUDA tensors) for
+        the same cparams / rparams, m <= 1024.  dir_c [K,Pc] / dir_r [K,Pr] are directions shared by the batch, [N,K,Pc] / [N,K,Pr] one
+        set per LP (either may be None: those parameters do not move); both None: the K = Pc + Pr coordinate axes, first every
+        cparam, then every rparam.  One kernel launch on torch's current stream, no synchronisation."""
+        import torch
+        t = self.t
+        if not torch.is_tensor(cparams) or not cparams.is_cuda or cparams.dtype != torch.float64 or cparams.dim() != 2 \
+                or cparams.shape[1] != t.Pc:
+            raise ValueError(f"cparams must be a CUDA float64 tensor of shape [N, {t.Pc}]")
+        N = cparams.shape[0]
+        dev = cparams.device
+        ok = lambda a, shape, dt: torch.is_tensor(a) and a.is_cuda and a.device == dev and a.is_contiguous() and tuple(a.shape) == shape \
+            and a.dtype == dt
+        if not (ok(vertex.status, (N,), torch.int32) and ok(vertex.col_status, (N, t.n), torch.int8)
+                and ok(vertex.row_basic, (N, t.m), torch.int8)):
+            raise ValueError(f"vertex.status / col_status / row_basic must be contiguous CUDA [{N}] int32, [{N}, {t.n}] and [{N}, {t.m}] "
+                             f"int8 tensors")
+        cparams = cparams.contiguous()
+        rstride, rptr = 0, None
+        if t.Pr:
+            if rparams is None or not torch.is_tensor(rparams) or not rparams.is_cuda or rparams.dtype != torch.float64 \
+                    or rparams.device != dev or tuple(rparams.shape) not in ((t.Pr,), (N, t.Pr)):
+                raise ValueError(f"rparams must be a CUDA float64 tensor of shape [{t.Pr}] or [{N}, {t.Pr}] on {dev}")
+            rparams = rparams.contiguous()
+            rstride = 0 if rparams.dim() == 1 else t.Pr
+            rptr = rparams.data_ptr()
+        if dir_c is None and dir_r is None:
+            K = t.Pc + t.Pr
+            dir_c = torch.eye(K, t.Pc, dtype=torch.float64, device=dev)
+            dir_r = torch.zeros((K, t.Pr), dtype=torch.float64, device=dev)
+            dir_r[t.Pc:] = torch.eye(t.Pr, dtype=torch.float64, device=dev)
+        dirs = [d for d in (dir_c, dir_r) if d is not None]
+        if not all(torch.is_tensor(d) and d.dim() in (2, 3) for d in dirs):
+            raise ValueError("dir_c / dir_r must be CUDA float64 tensors of shape [K, P] or [N, K, P]")
+        per_lp = dirs[0].dim() == 3
+        K = dirs[0].shape[-2]
+        for d, P, what in ((dir_c, t.Pc, "dir_c"), (dir_r, t.Pr, "dir_r")):
+            want = (N, K, P) if per_lp else (K, P)
+            if d is not None and (not torch.is_tensor(d) or not d.is_cuda or d.device != dev or d.dtype != torch.float64
+                                  or tuple(d.shape) != want):
+                raise ValueError(f"{what} must be a CUDA float64 tensor of shape {list(want)} on {dev}")
+        dir_c = dir_c.contiguous() if dir_c is not None else None
+        dir_r = dir_r.contiguous() if dir_r is not None else None
+        e = lambda shape, dt: torch.empty(shape, dtype=dt, device=dev)
+        out = Ranges(e((N, K), torch.float64), e((N, K), torch.float64), e((N, K), torch.float64), e((N, K), torch.float64),
+                     e((N,), torch.int32))
+        ptr = lambda a: a.data_ptr() if a is not None and a.numel() else None
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.dsp_lp_ranging(self.handle, N, ptr(cparams), rptr, rstride, vertex.status.data_ptr(), vertex.col_status.data_ptr(),
+                                     vertex.row_basic.data_ptr(), int(K), ptr(dir_c), ptr(dir_r), int(per_lp), ptr(out.theta_lo),
+                                     ptr(out.theta_hi), ptr(out.dobj), ptr(out.d2obj), ptr(out.status), C.c_void_p(stream))
+        self._check(rc, "dsp_lp_ranging")
         return out
 
     def crossover(self, cparams, rparams, result, max_pivots=0):

@@ -273,6 +273,42 @@ int dsp_lp_crossover(const dsp_template *t, int64_t N,
                      int8_t *col_status /*[N,n] or NULL*/, int8_t *row_basic /*[N,m] or NULL*/,
                      int32_t *xstatus /*[N]*/, int32_t *pivots /*[N] or NULL*/, void *cuda_stream);
 
+/* Ranging over given bases: for every LP and every direction k, the interval [theta_lo, theta_hi] (theta_lo <= 0 <= theta_hi, +-inf
+ * where unbounded) of theta over which the LP's basis stays optimal when the parameters move to (cp + theta dir_c[k], rp + theta
+ * dir_r[k]), all others fixed; Gurobi's SAObj* / SARHS* answer, for the batch parameters.  m <= 1024.
+ * The LP is dsp_lp_crossover's (caller's order, every per-problem parameter and matrix term) and so is the basis: col_status [N,n] and
+ * row_basic [N,m], e.g. dsp_lp_crossover's outputs with its status as xstatus.  Only the basis is read: x_B, y and d = c - A'y are
+ * recomputed from it.  The basis stays optimal while
+ *   primal: 0 <= x_B(theta) <= u_B(theta), u_j(theta) >= 0 for a nonbasic column at u, a basic artificial stays 0 (else [0, 0]);
+ *   dual:   d_j(theta) >= 0 at 0, <= 0 at u, for every nonbasic column except those fixed at 0 along the direction (u_j = 0 and no
+ *           change of u_j); nonbasic artificials impose nothing.  A column with u_j = 0 may sit at either bound, but where the
+ *           direction changes u_j and d_j has the wrong sign for its bound beyond tolerance, the side on which u_j grows is 0.
+ * An entry within the crossover's tolerance of its bound (1e-9 of the primal scale max(1, |b|_inf, |u_finite|_inf), of |c|_inf on the
+ * dual side) counts as on it: a direction pushing it outwards gives 0 on that side.  An entry whose rate of change is at most 1e-9 of
+ * the direction's scale (max(|Bmap dir_r|_inf, |Umap dir_r|_inf) on the primal side, |Cmap dir_c|_inf on the dual side) does not block.
+ * Inside the range obj(theta) = obj + dobj theta + d2obj theta^2 / 2 exactly; d2obj = 2 dc'dx is 0 unless the direction moves both c
+ * and b / u.  A direction with a nonzero dir_r entry on a parameter that enters a matrix term moves A: its column of every output is
+ * NaN.
+ * Directions: dir_c [K,Pc] and dir_r [K,Pr] shared by the batch (dir_stride == 0), or per LP [N,K,Pc] / [N,K,Pr] (dir_stride != 0);
+ * a NULL dir_c or dir_r does not move those parameters.
+ * rstatus [N]: DSP_OPTIMAL (ranges computed), DSP_NUMERICAL (the basis does not have m members or has a column at an infinite bound,
+ * its reinversion is singular, or it is not primal and dual feasible within the tolerances above at theta = 0), or the input xstatus
+ * where that is not DSP_OPTIMAL; every LP that is not DSP_OPTIMAL gets NaN rows.
+ * Algorithm (csrc/dsp_ranging.cuh, DESIGN.md 4.7): dsp_lp_crossover's layout, one CTA per LP, B^-1 by Gauss-Jordan, then per direction
+ * two dense m x m products and the ratio tests.  DEVICE pointers, stream-ordered, no synchronisation, the rparams_stride == 0
+ * broadcast of dsp_lp_solve_batch.  Results are bitwise reproducible and do not depend on where an LP sits in the batch.  One kernel
+ * launch per call (none when N == 0 or K == 0).
+ * DSP_E_ARG: NULL handle, N < 0, K < 0, m > 1024 ("ranging takes m <= 1024"), and for N > 0 and K > 0 NULL xstatus / col_status /
+ * row_basic / theta_lo / theta_hi / rstatus, NULL cparams with Pc > 0 or NULL rparams with Pr > 0. */
+int dsp_lp_ranging(const dsp_template *t, int64_t N,
+                   const double *cparams, const double *rparams, int64_t rparams_stride,
+                   const int32_t *xstatus, const int8_t *col_status, const int8_t *row_basic,
+                   int32_t K, const double *dir_c /*[K,Pc] or NULL*/, const double *dir_r /*[K,Pr] or NULL*/,
+                   int64_t dir_stride /* 0: directions shared by the batch; else per LP, [N,K,Pc] / [N,K,Pr] */,
+                   double *theta_lo /*[N,K]*/, double *theta_hi /*[N,K]*/,
+                   double *dobj /*[N,K] or NULL*/, double *d2obj /*[N,K] or NULL*/,
+                   int32_t *rstatus /*[N]*/, void *cuda_stream);
+
 /* Introspection used by tests / bench: kernel launches issued so far, last launch geometry (grid in CTAs, block, dynamic shared
  * memory; problems_per_cta: LPs per CTA, or for the dense cluster kernel the cluster size in CTAs). */
 int64_t dsp_lp_launch_count(void);
