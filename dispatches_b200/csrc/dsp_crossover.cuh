@@ -127,6 +127,15 @@ struct Shared {
 #define XO_SYNC() __syncthreads()
 #endif
 
+// the paths of lp_body, for XO_TRACE(ev): a test build counts them (tests/emu/emu_crossover.cpp); the library compiles the hook out
+enum {
+    TR_PUSH_PIVOT, TR_PUSH_REINVERT, TR_PRIMAL_PIVOT, TR_PRIMAL_DEGENERATE, TR_BOUND_FLIP, TR_DUAL_PIVOT, TR_BLAND,
+    TR_CLEANUP_REINVERT, TR_ARTIFICIAL_OUT, TR_REDUNDANT_ROW, TR_ROUND, TR_EVENTS
+};
+#ifndef XO_TRACE
+#define XO_TRACE(ev) ((void)0)
+#endif
+
 constexpr int kNone = 0x7fffffff;
 
 XOD bool better(double a1, double a2, int ai, double b1, double b2, int bi) {
@@ -567,8 +576,10 @@ XOD void lp_body(const Params &P, const sens::View &s, const View &X, double *w,
                 if (tid == 0) W.xv[j] = fma(step, (double)dir, x);
                 XO_SYNC();
                 pivot(W, m, n, k, j, to_up ? AT_UP : AT_LO, to_up ? upper(W, n, v) : 0.0, tid, nt);
+                XO_TRACE(TR_PUSH_PIVOT);
                 ++npiv; ++since;
                 if (since >= kRefactor) {
+                    XO_TRACE(TR_PUSH_REINVERT);
                     if (!reinvert(W, s, S, m, n, tid, nt)) status = NUMERICAL;
                     since = 0;
                     solve_x(W, X, m, n, false, tid, nt);
@@ -583,6 +594,7 @@ XOD void lp_body(const Params &P, const sens::View &s, const View &X, double *w,
     // ---- 3. and 4.: fresh inverse, cleanup pivots, artificials out, fresh inverse
     int degen = 0;
     for (int round = 0; round < 4 && status == OPTIMAL; ++round) {
+        XO_TRACE(TR_ROUND);
         if (!reinvert(W, s, S, m, n, tid, nt)) { status = NUMERICAL; break; }
         since = 0;
         solve_x(W, X, m, n, true, tid, nt);
@@ -603,6 +615,7 @@ XOD void lp_body(const Params &P, const sens::View &s, const View &X, double *w,
             if (pv != kNone && q != kNone) { status = NUMERICAL; break; }      // primal and dual infeasible
             if (npiv >= maxp) { status = MAX_ITER; break; }
             pivoted = true;
+            if (bland) XO_TRACE(TR_BLAND);
             if (q != kNone) {                            // bounded primal simplex
                 const int dir = W.stat[q] == AT_LO ? 1 : -1;
                 ftran(W, s, m, n, q, W.al, tid, nt);
@@ -613,10 +626,13 @@ XOD void lp_body(const Params &P, const sens::View &s, const View &X, double *w,
                 if (k == kNone || range <= theta) {      // bound flip
                     if (tid == 0) { W.stat[q] = dir > 0 ? AT_UP : AT_LO; W.xv[q] = dir > 0 ? range : 0.0; }
                     XO_SYNC();
+                    XO_TRACE(TR_BOUND_FLIP);
                     degen = 0;
                 } else {
                     const int v = W.head[k];
                     pivot(W, m, n, k, q, to_up ? AT_UP : AT_LO, to_up ? upper(W, n, v) : 0.0, tid, nt);
+                    XO_TRACE(TR_PRIMAL_PIVOT);
+                    if (theta == 0.0) XO_TRACE(TR_PRIMAL_DEGENERATE);
                     degen = theta == 0.0 ? degen + 1 : 0;
                     ++since;
                 }
@@ -632,11 +648,13 @@ XOD void lp_body(const Params &P, const sens::View &s, const View &X, double *w,
                 if (e == kNone) { status = NUMERICAL; break; }
                 ftran(W, s, m, n, e, W.al, tid, nt);
                 pivot(W, m, n, r, e, below ? AT_LO : AT_UP, below ? 0.0 : upper(W, n, pv), tid, nt);
+                XO_TRACE(TR_DUAL_PIVOT);
                 degen = ratio == 0.0 ? degen + 1 : 0;
                 ++since;
             }
             ++npiv;
             if (since >= kRefactor) {
+                XO_TRACE(TR_CLEANUP_REINVERT);
                 if (!reinvert(W, s, S, m, n, tid, nt)) { status = NUMERICAL; break; }
                 since = 0;
             }
@@ -653,11 +671,13 @@ XOD void lp_body(const Params &P, const sens::View &s, const View &X, double *w,
             const int ep = dual_ratio(W, S, n, 1, told, false, &rp_, tid, nt);
             const int en = dual_ratio(W, S, n, -1, told, false, &rn_, tid, nt);
             const int e = ep == kNone ? en : en == kNone ? ep : (rn_ < rp_ ? en : ep);
-            if (e == kNone) continue;                    // a redundant row: its artificial stays basic at 0
+            if (e == kNone) { XO_TRACE(TR_REDUNDANT_ROW); continue; }   // a redundant row: its artificial stays basic at 0
             ftran(W, s, m, n, e, W.al, tid, nt);
             pivot(W, m, n, r, e, AT_LO, 0.0, tid, nt);
+            XO_TRACE(TR_ARTIFICIAL_OUT);
             ++npiv; ++since; pivoted = true;
             if (since >= kRefactor) {
+                XO_TRACE(TR_CLEANUP_REINVERT);
                 if (!reinvert(W, s, S, m, n, tid, nt)) { status = NUMERICAL; break; }
                 since = 0;
             }

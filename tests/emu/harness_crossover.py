@@ -19,6 +19,12 @@ ROOT = HERE.parent.parent
 LIB = HERE / "libemu_crossover.so"
 _lib = None
 
+# the paths of xo::lp_body that XO_TRACE counts, in the order of dsp_crossover.cuh's TR_* events: push pivots and push reinversions;
+# cleanup primal pivots (degenerate ones also counted apart), bound flips, dual pivots, iterations under Bland's rule and reinversions;
+# artificials pivoted out, redundant rows met (an artificial that stays basic, once per round) and cleanup rounds
+TRACE = ("push_pivot", "push_reinvert", "primal_pivot", "primal_degenerate", "bound_flip", "dual_pivot", "bland", "cleanup_reinvert",
+         "artificial_out", "redundant_row", "round")
+
 
 def build(force=False):
     deps = [HERE / "emu_crossover.cpp", HERE / "simt_emu.h", ROOT / "dispatches_b200" / "csrc" / "dsp_crossover.cuh",
@@ -33,12 +39,14 @@ def build(force=False):
 
 
 def run(t, cparams, rparams, status, x, y, max_pivots=0, col_perm=None, row_perm=None):
-    """dict(obj, x, y, col_status, row_basic, status, pivots) of the emulated CTA body, x / y / basis in template order"""
+    """dict(obj, x, y, col_status, row_basic, status, pivots, trace) of the emulated CTA body, x / y / basis in template order;
+    trace: {path in TRACE: [N] times each LP took it}"""
     global _lib
     if _lib is None:
         _lib = C.CDLL(str(build()))
         _lib.emu_crossover.argtypes = [C.c_int] * 5 + [C.c_void_p] * 19 + [C.c_double, C.c_int] + [C.c_void_p] * 3 + \
-            [C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 7
+            [C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 8
+        assert _lib.emu_crossover_trace_events() == len(TRACE)
     I = internal(t, col_perm, row_perm)
     cperm = np.arange(t.n) if I["col_perm"] is None else I["col_perm"]
     rperm = np.arange(t.m) if I["row_perm"] is None else I["row_perm"]
@@ -59,6 +67,7 @@ def run(t, cparams, rparams, status, x, y, max_pivots=0, col_perm=None, row_perm
                 tc=f64(t.amap[3] if t.amap is not None else [0.0]), st=i32(status))
     out = dict(obj=np.empty(N), x=np.empty((N, t.n)), y=np.empty((N, t.m)), col_status=np.empty((N, t.n), np.int8),
                row_basic=np.empty((N, t.m), np.int8), status=np.empty(N, np.int32), pivots=np.empty(N, np.int32))
+    trace = np.zeros((N, len(TRACE)), np.int32)
     vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else None
     nt = len(t.amap[0]) if t.amap is not None else 0
     k = keep
@@ -67,6 +76,7 @@ def run(t, cparams, rparams, status, x, y, max_pivots=0, col_perm=None, row_perm
                            vp(k["u0"]), vp(k["ump"]), vp(k["umi"]), vp(k["umv"]), vp(k["om"]), vp(k["ocm"]), float(t.o0), nt,
                            vp(k["tq"]), vp(k["tp"]), vp(k["tc"]), N, vp(cp), vp(rp), rstride, vp(k["st"]), vp(x), vp(y), int(max_pivots),
                            vp(out["obj"]), vp(out["x"]), vp(out["y"]), vp(out["col_status"]), vp(out["row_basic"]), vp(out["status"]),
-                           vp(out["pivots"]))
+                           vp(out["pivots"]), vp(trace))
     assert r == 0
+    out["trace"] = {name: trace[:, q] for q, name in enumerate(TRACE)}
     return out

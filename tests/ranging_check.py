@@ -85,6 +85,11 @@ def exact_checks(s, k, basis, lo, hi, dobj, d2obj, dir_c, dir_r, what=""):
         if math.isfinite(side):
             past = side + sign * 1e-6 * max(abs(side), p)
             c3, r3 = XR.moved(t, cp, rp, dir_c, dir_r, past)
+            u3 = t.instantiate(c3, r3 if r3 is not None else np.zeros(0))[2]
+            if ((u3 < 0) & (t.instantiate(cp, rp if rp is not None else np.zeros(0))[2] >= 0)).any():
+                # the side where an upper bound reaches 0: past it the LP has no feasible point, so no basis is optimal there (the
+                # kernels clip a negative bound to 0, the LP verify() checks, on which the basis can stay optimal)
+                continue
             try:
                 XR.verify(t, c3, r3, basis)
             except E.NotCertified:
