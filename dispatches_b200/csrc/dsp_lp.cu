@@ -1150,6 +1150,23 @@ __global__ void __launch_bounds__(kXoThreads) dsp_lp_ranging_kernel(const rg::Pa
     for (long long p = blockIdx.x; p < P.N; p += gridDim.x) rg::lp_body(P, v, X, w, &S, p, threadIdx.x, blockDim.x);
 }
 
+}  // namespace
+
+#include "dsp_parametric.cuh"
+
+namespace {
+// parametric walk (dsp_parametric.cuh): the crossover's geometry, one (LP, direction) pair per CTA, its work region in dynamic shared
+// memory when it fits, else in the handle's workspace
+__global__ void __launch_bounds__(kXoThreads) dsp_lp_parametric_kernel(const pm::Params P) {
+    extern __shared__ __align__(16) double pm_smem[];
+    __shared__ xo::Shared S;
+    double *w = P.ws ? P.ws + (long long)blockIdx.x * P.ws_stride : pm_smem;
+    const sens::View v = sens::view_of(P.blob, P.L);
+    const xo::View X = xo::view_of(P.xblob, P.X);
+    const long long pairs = P.N * P.K;
+    for (long long pk = blockIdx.x; pk < pairs; pk += gridDim.x) pm::pair_body(P, v, X, w, &S, pk, threadIdx.x, blockDim.x);
+}
+
 // FP64 FMA micro-benchmark: the measured denominator of the FP64 roofline fraction bench.py reports.  8 independent DFMA
 // chains per thread.
 __global__ void __launch_bounds__(256) dsp_fp64_peak_kernel(double *out, int iters, double a, double b) {
@@ -2300,6 +2317,51 @@ int dsp_lp_ranging(const dsp_template *T, int64_t N, const double *cparams, cons
     if (int rc = xo_grid(T, dsp_lp_ranging_kernel, N, rg::work_doubles(K.m, K.n, P.nnz), st, &g)) return rc;
     P.ws = g.ws; P.ws_stride = g.ws_stride;
     dsp_lp_ranging_kernel<<<(unsigned)g.blocks, kXoThreads, g.smem, st>>>(P);
+    return launched(g.blocks, kXoThreads, g.smem, 1);
+}
+
+int dsp_lp_parametric(const dsp_template *T, int64_t N, const double *cparams, const double *rparams, int64_t rparams_stride,
+                      const int32_t *xstatus, const int8_t *col_status, const int8_t *row_basic, int32_t Kd, const double *dir_c,
+                      const double *dir_r, int64_t dir_stride, const double *theta_end, int32_t S, double *theta, double *obj,
+                      double *dobj, double *d2obj, int32_t *enter, int32_t *leave, int8_t *leave_to, int32_t *count, int32_t *pstatus,
+                      void *cuda_stream) {
+    if (!T) { g_err = "dsp_lp_parametric: null handle"; return DSP_E_ARG; }
+    if (N < 0) { g_err = "dsp_lp_parametric: N < 0"; return DSP_E_ARG; }
+    if (Kd < 0) { g_err = "dsp_lp_parametric: K < 0"; return DSP_E_ARG; }
+    if (S < 1) { g_err = "dsp_lp_parametric: S < 1"; return DSP_E_ARG; }
+    if (T->kp.m > 1024) { g_err = "dsp_lp_parametric: parametric takes m <= 1024"; return DSP_E_ARG; }
+    if (N == 0 || Kd == 0) return 0;
+    if (!xstatus || !col_status || !row_basic) { g_err = "dsp_lp_parametric: xstatus, col_status and row_basic are required"; return DSP_E_ARG; }
+    if (!theta || !obj || !dobj || !count || !pstatus) {
+        g_err = "dsp_lp_parametric: theta, obj, dobj, count and pstatus are required"; return DSP_E_ARG;
+    }
+    if (!theta_end) { g_err = "dsp_lp_parametric: theta_end is required"; return DSP_E_ARG; }
+    if (T->kp.Pc > 0 && !cparams) { g_err = "dsp_lp_parametric: cparams is NULL but the template has Pc > 0"; return DSP_E_ARG; }
+    if (T->kp.Pr > 0 && !rparams) { g_err = "dsp_lp_parametric: rparams is NULL but the template has Pr > 0"; return DSP_E_ARG; }
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    {                                  // theta_end: every entry >= 0 (+inf allowed), read back on the stream
+        const size_t ne = (size_t)(dir_stride != 0 ? N * (int64_t)Kd : Kd);
+        std::vector<double> te(ne);
+        CK(cudaMemcpyAsync(te.data(), theta_end, ne * sizeof(double), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        for (double v : te)
+            if (!(v >= 0.0)) { g_err = "dsp_lp_parametric: theta_end must be >= 0 (not NaN) in every entry"; return DSP_E_ARG; }
+    }
+    if (int e = ensure_xo(T)) return e;
+    const KParams &K = T->kp;
+    pm::Params P;
+    P.m = K.m; P.n = K.n; P.Pc = K.Pc; P.Pr = K.Pr; P.nnz = T->band.A_ptr[K.m]; P.K = Kd; P.S = S;
+    P.N = N; P.cparams = cparams; P.rparams = rparams; P.rstride = rparams_stride;
+    P.status = xstatus; P.col_status = (const signed char *)col_status; P.row_basic = (const signed char *)row_basic;
+    P.dir_c = K.Pc > 0 ? dir_c : nullptr; P.dir_r = K.Pr > 0 ? dir_r : nullptr; P.dir_per_lp = dir_stride != 0;
+    P.theta_end = theta_end; P.o0 = K.o0;
+    P.theta = theta; P.obj = obj; P.dobj = dobj; P.d2obj = d2obj; P.enter = enter; P.leave = leave; P.leave_to = (signed char *)leave_to;
+    P.count = count; P.pstatus = pstatus;
+    P.blob = T->sns.blob; P.L = T->sns.L; P.xblob = T->xov.blob; P.X = T->xov.L;
+    XoGrid g;
+    if (int rc = xo_grid(T, dsp_lp_parametric_kernel, N * (long long)Kd, pm::work_doubles(K.m, K.n, P.nnz, K.Pc, K.Pr), st, &g)) return rc;
+    P.ws = g.ws; P.ws_stride = g.ws_stride;
+    dsp_lp_parametric_kernel<<<(unsigned)g.blocks, kXoThreads, g.smem, st>>>(P);
     return launched(g.blocks, kXoThreads, g.smem, 1);
 }
 

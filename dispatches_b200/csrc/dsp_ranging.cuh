@@ -22,6 +22,7 @@
 //      obj(theta) = obj + dobj theta + d2obj theta^2 / 2 with dobj = dc'x + c'dx + omap'dir_r + ocmap'dir_c and d2obj = 2 dc'dx.
 //      A direction with a nonzero dir_r entry on a parameter that enters a matrix term gets NaN in all four outputs: A moves and the
 //      objective is not piecewise quadratic along it.
+//      Step 3 is rg::segment, which the parametric walk (dsp_parametric.cuh) calls for every segment of its walk.
 //
 // Layout: the crossover's (dsp_crossover.cuh): one CTA per LP, LPs handed out grid-stride, the work region (B^-1, the LP's vectors and
 // the direction's) in shared memory or in the handle's workspace.  Every element is summed by one thread in a fixed order and every
@@ -59,11 +60,17 @@ struct Params {
 // doubles of one LP's work region: the crossover's, then dc, du, dx (n each), db, dy (m each)
 XOHD long long work_doubles(int m, int n, int nnz) { return xo::work_doubles(m, n, nnz) + (3LL * n + 2LL * m + 1) / 2 * 2; }
 
-// the tighter of the two sides g + theta dg >= 0 may block: into *hi when dg < 0, into *lo (as a distance) when dg > 0
-XOD void block(double g, double dg, double tol, double rtol, double *hi, double *lo) {
+// block kinds of the upper side (for the parametric walk, dsp_parametric.cuh): a basic column reaching 0 or its u, a basic artificial
+// leaving 0, a nonbasic column at u whose u reaches 0, a reduced cost reaching 0, a fixed column unfixed at the wrong bound
+enum { BK_BASIC_LO = 0, BK_BASIC_UP = 1, BK_ARTIFICIAL = 2, BK_BOUND = 3, BK_DUAL = 4, BK_UNFIX = 5 };
+
+// the tighter of the two sides g + theta dg >= 0 may block: into *hi when dg < 0, into *lo (as a distance) when dg > 0.  The upper
+// side keeps its blocking entry, the smallest (ratio, class, id) with id = variable * 8 + kind and class -1 for a fixed column
+// unfixed at the wrong bound (a flip that changes no value), 0 for a primal entry, 1 for a dual one
+XOD void block(double g, double dg, double tol, double rtol, double *hi, double *lo, double *hc, int *hid, double cls, int id) {
     if (!(fabs(dg) > rtol)) return;
     const double r = g <= tol ? 0.0 : g / fabs(dg);
-    if (dg < 0.0) *hi = fmin(*hi, r);
+    if (dg < 0.0) xo::keep_best(*hi, *hc, *hid, r, cls, id);
     else *lo = fmin(*lo, r);
 }
 
@@ -71,6 +78,116 @@ XOD void block(double g, double dg, double tol, double rtol, double *hi, double 
 XOD double block_max(xo::Shared *S, int tid, int nt, double v) {
     xo::choose(S, tid, nt, -v, 0.0, 0);
     return -S->r1;
+}
+
+// one range of a basis along a direction: hi / lo as distances from the current point, the blocking entry of the upper side
+// (variable * 8 + kind, xo::kNone where nothing blocks), and (thread 0 only) the objective's first and second derivative
+struct Segment { double hi, lo, d1, d2; int block; };
+
+// step 3 for the direction (gc, gr) on the current basis, x_B, y and d: dc, du, db, dy, dd = dc - A'dy and dx of every column (dx_B
+// also in W.al), then the ratio tests.  tolp / told: the on-bound tolerances.
+XOD Segment segment(const sens::View &s, const xo::View &X, const xo::Work &W, xo::Shared *S, int m, int n, int Pc, int Pr,
+                    const double *gc, const double *gr, double *dc, double *du, double *dx, double *db, double *dy, double *dd,
+                    double tolp, double told, int tid, int nt) {
+    double sdp = 0.0, sdd = 0.0;
+    for (int j = tid; j < n; j += nt) {
+        double v = 0.0;
+        if (gc)
+            for (int e = sens::ld<true>(s.cm_ptr + j), e1 = sens::ld<true>(s.cm_ptr + j + 1); e < e1; ++e)
+                v = fma(sens::ld<true>(s.cm_val + e), gc[sens::ld<true>(s.cm_idx + e)], v);
+        dc[j] = v;
+        double g = 0.0;
+        if (gr && sens::ld<true>(X.u0 + j) < INFINITY)
+            for (int e = sens::ld<true>(X.um_ptr + j), e1 = sens::ld<true>(X.um_ptr + j + 1); e < e1; ++e)
+                g = fma(sens::ld<true>(X.um_val + e), gr[sens::ld<true>(X.um_idx + e)], g);
+        du[j] = g;
+        sdd = fmax(sdd, fabs(v)); sdp = fmax(sdp, fabs(g));
+    }
+    for (int i = tid; i < m; i += nt) {
+        double v = 0.0;
+        if (gr)
+            for (int e = sens::ld<true>(X.bm_ptr + i), e1 = sens::ld<true>(X.bm_ptr + i + 1); e < e1; ++e)
+                v = fma(sens::ld<true>(X.bm_val + e), gr[sens::ld<true>(X.bm_idx + e)], v);
+        db[i] = v;
+        sdp = fmax(sdp, fabs(v));
+    }
+    sdp = block_max(S, tid, nt, sdp);
+    sdd = block_max(S, tid, nt, sdd);
+    // dy = B^-T dc_B, dd = dc - A'dy; the right-hand side of dx_B (into t1)
+    for (int q = tid; q < m; q += nt) W.t2[q] = W.head[q] < n ? dc[W.head[q]] : 0.0;
+    for (int i = tid; i < m; i += nt) {
+        double r = db[i];
+        for (int q = sens::ld<true>(X.r_ptr + i), q1 = sens::ld<true>(X.r_ptr + i + 1); q < q1; ++q) {
+            const int j = sens::ld<true>(X.r_col + q);
+            if (W.stat[j] == xo::AT_UP) r = fma(-W.a[sens::ld<true>(X.r_pos + q)], du[j], r);
+        }
+        W.t1[i] = r;
+    }
+    XO_SYNC();
+    for (int i = tid; i < m; i += nt) {
+        double r = 0.0;
+        for (int q = 0; q < m; ++q) r = fma(W.t2[q], W.B[(long long)q * m + i], r);
+        dy[i] = r;
+    }
+    for (int q = tid; q < m; q += nt) {
+        double r = 0.0;
+        for (int i = 0; i < m; ++i) r = fma(W.B[(long long)q * m + i], W.t1[i], r);
+        W.al[q] = r;
+    }
+    XO_SYNC();
+    for (int j = tid; j < n; j += nt) {
+        dd[j] = dc[j] - xo::col_dot(W, s, n, j, dy);
+        dx[j] = W.stat[j] == xo::AT_UP ? du[j] : 0.0;
+    }
+    XO_SYNC();
+    for (int q = tid; q < m; q += nt) if (W.head[q] < n) dx[W.head[q]] = W.al[q];
+    // the ratio tests: hi and lo as distances from 0
+    const double rtp = kRate * sdp, rtd = kRate * sdd;
+    double hi = INFINITY, lo = INFINITY, hc = 0.0;
+    int hid = xo::kNone;
+    for (int q = tid; q < m; q += nt) {
+        const int v = W.head[q];
+        const double x = W.xv[v], g = W.al[q];
+        if (v >= n) {
+            if (fabs(g) > rtp) { xo::keep_best(hi, hc, hid, 0.0, 0.0, v * 8 + BK_ARTIFICIAL); lo = 0.0; }
+            continue;
+        }
+        block(x, g, tolp, rtp, &hi, &lo, &hc, &hid, 0.0, v * 8 + BK_BASIC_LO);
+        if (W.u[v] < INFINITY) block(W.u[v] - x, du[v] - g, tolp, rtp, &hi, &lo, &hc, &hid, 0.0, v * 8 + BK_BASIC_UP);
+    }
+    for (int j = tid; j < n; j += nt) {
+        const int st = W.stat[j];
+        if (st == xo::BASIC) continue;
+        if (st == xo::AT_UP) block(W.u[j], du[j], tolp, rtp, &hi, &lo, &hc, &hid, 0.0, j * 8 + BK_BOUND);
+        if (W.u[j] <= 0.0) {         // fixed at 0 at theta = 0, its bound free of the sign of d_j
+            if (du[j] == 0.0) continue;
+            if ((st == xo::AT_LO ? W.d[j] : -W.d[j]) < -told) {     // at the wrong bound: optimal only while u_j stays 0
+                if (du[j] > 0.0) xo::keep_best(hi, hc, hid, 0.0, -1.0, j * 8 + BK_UNFIX);
+                else lo = 0.0;
+                continue;
+            }
+        }
+        if (st == xo::AT_LO) block(W.d[j], dd[j], told, rtd, &hi, &lo, &hc, &hid, 1.0, j * 8 + BK_DUAL);
+        else block(-W.d[j], -dd[j], told, rtd, &hi, &lo, &hc, &hid, 1.0, j * 8 + BK_DUAL);
+    }
+    Segment g;
+    xo::choose(S, tid, nt, hi, hc, hid);
+    g.hi = S->r1; g.block = S->rid;
+    xo::choose(S, tid, nt, lo, 0.0, 0);
+    g.lo = S->r1;
+    g.d1 = g.d2 = 0.0;
+    if (tid == 0) {
+        double d1 = 0.0, d2 = 0.0;
+        for (int j = 0; j < n; ++j) {
+            d1 = fma(dc[j], W.xv[j], d1);
+            d1 = fma(W.c[j], dx[j], d1);
+            d2 = fma(dc[j], dx[j], d2);
+        }
+        if (gr) for (int q = 0; q < Pr; ++q) d1 = fma(sens::ld<true>(s.omap + q), gr[q], d1);
+        if (gc) for (int q = 0; q < Pc; ++q) d1 = fma(sens::ld<true>(s.ocmap + q), gc[q], d1);
+        g.d1 = d1; g.d2 = 2.0 * d2;
+    }
+    return g;
 }
 
 // the outputs of LP p, computed by the threads tid = 0 .. nt-1 of one CTA (nt <= xo::kMaxThreads); w: the LP's work region
@@ -181,102 +298,11 @@ XOD void lp_body(const Params &P, const sens::View &s, const xo::View &X, double
             XO_SYNC();
             continue;
         }
-        double sdp = 0.0, sdd = 0.0;
-        for (int j = tid; j < n; j += nt) {
-            double v = 0.0;
-            if (gc)
-                for (int e = sens::ld<true>(s.cm_ptr + j), e1 = sens::ld<true>(s.cm_ptr + j + 1); e < e1; ++e)
-                    v = fma(sens::ld<true>(s.cm_val + e), gc[sens::ld<true>(s.cm_idx + e)], v);
-            dc[j] = v;
-            double g = 0.0;
-            if (gr && sens::ld<true>(X.u0 + j) < INFINITY)
-                for (int e = sens::ld<true>(X.um_ptr + j), e1 = sens::ld<true>(X.um_ptr + j + 1); e < e1; ++e)
-                    g = fma(sens::ld<true>(X.um_val + e), gr[sens::ld<true>(X.um_idx + e)], g);
-            du[j] = g;
-            sdd = fmax(sdd, fabs(v)); sdp = fmax(sdp, fabs(g));
-        }
-        for (int i = tid; i < m; i += nt) {
-            double v = 0.0;
-            if (gr)
-                for (int e = sens::ld<true>(X.bm_ptr + i), e1 = sens::ld<true>(X.bm_ptr + i + 1); e < e1; ++e)
-                    v = fma(sens::ld<true>(X.bm_val + e), gr[sens::ld<true>(X.bm_idx + e)], v);
-            db[i] = v;
-            sdp = fmax(sdp, fabs(v));
-        }
-        sdp = block_max(S, tid, nt, sdp);
-        sdd = block_max(S, tid, nt, sdd);
-        // dy = B^-T dc_B, dd = dc - A'dy (into alr); the right-hand side of dx_B (into t1)
-        for (int q = tid; q < m; q += nt) W.t2[q] = W.head[q] < n ? dc[W.head[q]] : 0.0;
-        for (int i = tid; i < m; i += nt) {
-            double r = db[i];
-            for (int q = sens::ld<true>(X.r_ptr + i), q1 = sens::ld<true>(X.r_ptr + i + 1); q < q1; ++q) {
-                const int j = sens::ld<true>(X.r_col + q);
-                if (W.stat[j] == xo::AT_UP) r = fma(-W.a[sens::ld<true>(X.r_pos + q)], du[j], r);
-            }
-            W.t1[i] = r;
-        }
-        XO_SYNC();
-        for (int i = tid; i < m; i += nt) {
-            double r = 0.0;
-            for (int q = 0; q < m; ++q) r = fma(W.t2[q], W.B[(long long)q * m + i], r);
-            dy[i] = r;
-        }
-        for (int q = tid; q < m; q += nt) {
-            double r = 0.0;
-            for (int i = 0; i < m; ++i) r = fma(W.B[(long long)q * m + i], W.t1[i], r);
-            W.al[q] = r;
-        }
-        XO_SYNC();
-        for (int j = tid; j < n; j += nt) {
-            W.alr[j] = dc[j] - xo::col_dot(W, s, n, j, dy);
-            dx[j] = W.stat[j] == xo::AT_UP ? du[j] : 0.0;
-        }
-        XO_SYNC();
-        for (int q = tid; q < m; q += nt) if (W.head[q] < n) dx[W.head[q]] = W.al[q];
-        // the ratio tests: hi and lo as distances from 0
-        const double rtp = kRate * sdp, rtd = kRate * sdd;
-        double hi = INFINITY, lo = INFINITY;
-        for (int q = tid; q < m; q += nt) {
-            const int v = W.head[q];
-            const double x = W.xv[v], g = W.al[q];
-            if (v >= n) {
-                if (fabs(g) > rtp) hi = lo = 0.0;
-                continue;
-            }
-            block(x, g, tolp, rtp, &hi, &lo);
-            if (W.u[v] < INFINITY) block(W.u[v] - x, du[v] - g, tolp, rtp, &hi, &lo);
-        }
-        for (int j = tid; j < n; j += nt) {
-            const int st = W.stat[j];
-            if (st == xo::BASIC) continue;
-            if (st == xo::AT_UP) block(W.u[j], du[j], tolp, rtp, &hi, &lo);
-            if (W.u[j] <= 0.0) {         // fixed at 0 at theta = 0, its bound free of the sign of d_j
-                if (du[j] == 0.0) continue;
-                if ((st == xo::AT_LO ? W.d[j] : -W.d[j]) < -told) {     // at the wrong bound: optimal only while u_j stays 0
-                    if (du[j] > 0.0) hi = 0.0;
-                    else lo = 0.0;
-                    continue;
-                }
-            }
-            if (st == xo::AT_LO) block(W.d[j], W.alr[j], told, rtd, &hi, &lo);
-            else block(-W.d[j], -W.alr[j], told, rtd, &hi, &lo);
-        }
-        xo::choose(S, tid, nt, hi, 0.0, 0);
-        hi = S->r1;
-        xo::choose(S, tid, nt, lo, 0.0, 0);
-        lo = S->r1;
+        const Segment g = segment(s, X, W, S, m, n, P.Pc, P.Pr, gc, gr, dc, du, dx, db, dy, W.alr, tolp, told, tid, nt);
         if (tid == 0) {
-            double d1 = 0.0, d2 = 0.0;
-            for (int j = 0; j < n; ++j) {
-                d1 = fma(dc[j], W.xv[j], d1);
-                d1 = fma(W.c[j], dx[j], d1);
-                d2 = fma(dc[j], dx[j], d2);
-            }
-            if (gr) for (int q = 0; q < P.Pr; ++q) d1 = fma(sens::ld<true>(s.omap + q), gr[q], d1);
-            if (gc) for (int q = 0; q < P.Pc; ++q) d1 = fma(sens::ld<true>(s.ocmap + q), gc[q], d1);
-            P.lo[p * K + k] = 0.0 - lo; P.hi[p * K + k] = hi;
-            if (P.dobj) P.dobj[p * K + k] = d1;
-            if (P.d2obj) P.d2obj[p * K + k] = 2.0 * d2;
+            P.lo[p * K + k] = 0.0 - g.lo; P.hi[p * K + k] = g.hi;
+            if (P.dobj) P.dobj[p * K + k] = g.d1;
+            if (P.d2obj) P.d2obj[p * K + k] = g.d2;
         }
         XO_SYNC();
     }

@@ -70,6 +70,9 @@ class PriceTakerResult:
     # "h2_price_per_kg" [N,2] where the case has them.  Inside an interval the objective is linear in that parameter.  NaN rows for
     # an LP whose crossover did not end OPTIMAL (it keeps its interior-point solution).
     ranges: dict | None = None
+    # want_curves={name: end}: the exact objective along each parameter from its input value up to `end` (include/dsp_lp.h:
+    # dsp_lp_parametric), a Curve per name in absolute units
+    curves: dict | None = None
 
     @property
     def NPV(self):
@@ -120,6 +123,81 @@ class PriceTakerResult:
         return pe.sum(1) * TP.PEM_ELEC_TO_MOL / TP.H2_MOLS_PER_KG * 3600.0 * self.sizes["h2_price"] * ann
 
 
+@dataclasses.dataclass
+class Curve:
+    """one parameter's exact curve per LP (per LP and hour for "lmp": [N,T,S] where below says [N,S]), from the parametric walk of the
+    returned vertex: events at parameter values `at`, the curve's value there and its right slope / curvature, in the case's units
+    (renewables: NPV in $ against MW, $/MWh or $/kg; nuclear: the objective).  Between events
+    npv(p) = npv[e] + slope[e] (p - at[e]) + curvature[e] (p - at[e])^2 / 2; entries from count on are NaN."""
+    at: np.ndarray          # [N(,T),S] parameter values of the events (the first is the input value)
+    npv: np.ndarray         # [N(,T),S] NPV (nuclear: the objective) there
+    slope: np.ndarray       # [N(,T),S] d npv / d parameter on the segment each event opens
+    curvature: np.ndarray   # [N(,T),S]
+    count: np.ndarray       # [N(,T)] events
+    status: np.ndarray      # [N(,T)] OPTIMAL (the walk reached `end`), INFEASIBLE / UNBOUNDED (the curve stops at its last event),
+    #                         MAX_ITER, NUMERICAL, or the LP's status where its crossover did not end OPTIMAL (count 0)
+    end: np.ndarray         # [N(,T)] the requested end
+
+    def value(self, p):
+        """the curve at absolute parameter values p (scalar, [P], or [N(,T),P]) -> [N(,T),P]; NaN outside [at[0], end], past the
+        last event of a walk that did not end OPTIMAL, and where the walk has no events"""
+        at = self.at
+        p = np.atleast_1d(np.asarray(p, float))
+        p = np.broadcast_to(p if p.ndim == at.ndim else p.reshape((1,) * (at.ndim - 1) + (-1,)), at.shape[:-1] + (p.shape[-1],))
+        stops = (self.status == 3) | (self.status == 4)
+        last = self.count - stops                                       # events that open a segment
+        S = at.shape[-1]
+        key = np.where(np.arange(S) < last[..., None], at, np.inf)
+        e = np.empty(p.shape, int)
+        for idx in np.ndindex(at.shape[:-1]):
+            e[idx] = np.searchsorted(key[idx], p[idx], side="right") - 1
+        e = np.clip(e, 0, S - 1)
+        g = lambda a: np.take_along_axis(a, e, axis=-1)
+        d = p - g(at)
+        with np.errstate(invalid="ignore"):
+            out = g(self.npv) + g(self.slope) * d + 0.5 * g(self.curvature) * d * d
+        lastat = np.take_along_axis(at, np.clip(self.count - 1, 0, S - 1)[..., None], axis=-1)
+        bad = (last[..., None] < 1) | (p < at[..., :1]) | (p > self.end[..., None]) | ((self.status != OPTIMAL)[..., None] & (p > lastat))
+        return np.where(bad, np.nan, out)
+
+
+def _walk_ends(name, value, end, N):
+    """theta_end of the walk from value (absolute, [N] or [N,T]) up to end; ValueError below the input value"""
+    end = np.broadcast_to(np.asarray(end, float), np.shape(value))
+    if np.isnan(end).any() or (end < value).any():
+        raise ValueError(f"want_curves[{name!r}]: the end must be at least the input value ({np.min(value)} ..)")
+    return end - value, end
+
+
+def _curve(c, k, value, end, scale):
+    """Curve of walk directions k of a Curves (host arrays [N,K,S]) starting at value [N(,T)]; npv = scale * obj"""
+    sl = lambda a: a[:, k]                                # k: one direction index ([N,S]) or T of them ([N,T,S])
+    th = sl(c["theta"])
+    return Curve(at=value[..., None] + th, npv=scale * sl(c["obj"]), slope=scale * sl(c["dobj"]), curvature=scale * sl(c["d2obj"]),
+                 count=sl(c["count"]), status=sl(c["status"]), end=np.broadcast_to(end, value.shape).copy())
+
+
+def _curve_directions(T, cf, N, names, values, pem=False):
+    """(dir_c [N,K,Pc], dir_r [N,K,Pr], theta_end [N,K], {name: direction indices}) of wind_battery(_pem) for the names of
+    want_curves: "lmp" T directions (1 $/MWh each), "h2_price_per_kg" (1 $/kg), "wind_mw" / "batt_mw" / "pem_mw" (1 MW, as
+    _wind_directions)"""
+    dc_all, dr_all = _wind_directions(T, cf, N, pem=pem)
+    Pc = T + pem
+    col = dict(lmp=list(range(T)), wind_mw=[Pc], batt_mw=[Pc + 1])
+    if pem:
+        col.update(h2_price_per_kg=[T], pem_mw=[Pc + 2])
+    ks, where, te, ends = [], {}, [], {}
+    for name, end in names.items():
+        if name not in col:
+            raise ValueError(f"want_curves: unknown name {name!r} (known: {sorted(col)})")
+        v = values[name]
+        th, ends[name] = _walk_ends(name, v, end, N)
+        where[name] = list(range(len(ks), len(ks) + len(col[name])))
+        ks += col[name]
+        te.append(th.reshape(N, -1))
+    return dc_all[:, ks], dr_all[:, ks], np.concatenate(te, axis=1), where, ends
+
+
 def _lmps(input_params, T):
     lmp = np.asarray(input_params["DA_LMPs"], float)
     lmp = np.atleast_2d(lmp)[:, :T]
@@ -128,29 +206,34 @@ def _lmps(input_params, T):
     return np.ascontiguousarray(lmp)
 
 
-def _solve_on_device(sol, cp, rp, want_sensitivities=False, directions=None):
+def _solve_on_device(sol, cp, rp, want_sensitivities=False, directions=None, walks=None, max_events=256):
     """the batch through the device path on cuda:0 (dsp_lp_solve_batch with x and y); with directions (dir_c [N,K,Pc], dir_r [N,K,Pr]
     or None) also dsp_lp_crossover, whose vertex replaces the interior point of every LP it takes OPTIMAL, and dsp_lp_ranging of that
-    basis; with want_sensitivities dsp_lp_sensitivities at the returned (x, y).  numpy results: (LPResult, d_cparams, d_rparams,
-    theta_lo, theta_hi), None where not asked for"""
+    basis; with walks (dir_c, dir_r, theta_end [N,K]) dsp_lp_parametric from the same vertex (one crossover serves both); with
+    want_sensitivities dsp_lp_sensitivities at the returned (x, y).  numpy results: (LPResult, d_cparams, d_rparams, theta_lo,
+    theta_hi, curves), None where not asked for"""
     import torch
     dev = torch.device("cuda", 0)
     cpt = torch.as_tensor(np.ascontiguousarray(cp, float), device=dev)
     rpt = torch.as_tensor(np.ascontiguousarray(rp, float), device=dev) if rp is not None else None
     host = lambda a: a.cpu().numpy()
     r = sol.solve(cpt, rpt, want_x=True, want_y=True)
-    lo = hi = dc = dr = None
-    if directions is not None:
+    lo = hi = dc = dr = curves = None
+    if directions is not None or walks is not None:
         v = sol.crossover(cpt, rpt, r)
         ok = v.status == OPTIMAL
         r = LPResult(torch.where(ok, v.obj, r.obj), r.status, r.iters, torch.where(ok[:, None], v.x, r.x), torch.where(ok[:, None], v.y, r.y))
-        gc, gr = (None if d is None else torch.as_tensor(np.ascontiguousarray(d, float), device=dev) for d in directions)
-        g = sol.ranging(cpt, rpt, v, gc, gr)
-        lo, hi = host(g.theta_lo), host(g.theta_hi)
+        dev_ = lambda d: None if d is None else torch.as_tensor(np.ascontiguousarray(d, float), device=dev)
+        if directions is not None:
+            g = sol.ranging(cpt, rpt, v, *(dev_(d) for d in directions))
+            lo, hi = host(g.theta_lo), host(g.theta_hi)
+        if walks is not None:
+            w = sol.parametric(cpt, rpt, v, dev_(walks[0]), dev_(walks[1]), theta_end=dev_(walks[2]), max_events=max_events)
+            curves = {f: host(getattr(w, f)) for f in ("theta", "obj", "dobj", "d2obj", "count", "status")}
     if want_sensitivities:
         g = sol.sensitivities(cpt, rpt, r, want_rc=False)
         dc, dr = host(g.d_cparams), host(g.d_rparams)
-    return LPResult(host(r.obj), host(r.status), host(r.iters), host(r.x), host(r.y)), dc, dr, lo, hi
+    return LPResult(host(r.obj), host(r.status), host(r.iters), host(r.x), host(r.y)), dc, dr, lo, hi, curves
 
 
 def _wind_directions(T, cf, N, pem=False):
@@ -187,6 +270,22 @@ def _wind_ranges(T, lmp, input_params, lo, hi, h2=None):
     return out
 
 
+def _wind_walks(T, cf, N, lmp, input_params, want_curves, h2=None):
+    """(dir_c, dir_r, theta_end, where, starts, ends) of the want_curves walks of wind_battery(_pem)"""
+    size = lambda key: np.broadcast_to(np.asarray(input_params[key], float), (N,)).copy()
+    values = dict(lmp=lmp, wind_mw=size("wind_mw"), batt_mw=size("batt_mw"))
+    if h2 is not None:
+        values.update(pem_mw=size("pem_mw"), h2_price_per_kg=np.asarray(h2, float))
+    dc, dr, te, where, ends = _curve_directions(T, cf, N, dict(want_curves), values, pem=h2 is not None)
+    return dc, dr, te, where, values, ends
+
+
+def _wind_curves(c, walks):
+    """PriceTakerResult.curves of wind_battery(_pem): NPV = -1e5 obj"""
+    _, _, _, where, values, ends = walks
+    return {name: _curve(c, k if name == "lmp" else k[0], values[name], ends[name], -1e5) for name, k in where.items()}
+
+
 def _wind_marginals(T, cf, dc, dr, N, pem=False):
     """d NPV / d sizes and prices of wind_battery(_pem): rparams = [wind_kw cf_t (T), batt_kw, wind_kw(, pem_kw)], cparams = [lmp(, h2)]"""
     cf = np.broadcast_to(np.asarray(cf, float), (N, T))
@@ -197,14 +296,19 @@ def _wind_marginals(T, cf, dc, dr, N, pem=False):
 
 
 def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solution=True, kernel=None, want_sensitivities=False,
-                          want_ranges=False):
+                          want_ranges=False, want_curves=None, max_events=256):
     """kernel: a solver.KERNEL_* choice for the band-template paths (None: the library's default, e.g. KERNEL_BAND_SPLIT for a long
     horizon on the split band kernel); the free-wind design (per-problem matrix coefficients) does not take it.
     want_sensitivities (fixed design only): fill PriceTakerResult.marginal_npv (wind_mw, batt_mw, lmp).
     want_ranges (fixed design only, templates of up to 1024 rows): solve, cross over to a vertex and fill PriceTakerResult.ranges
-    (lmp, wind_mw, batt_mw); the returned schedule is the vertex (and marginal_npv, when asked for, its gradient)."""
+    (lmp, wind_mw, batt_mw); the returned schedule is the vertex (and marginal_npv, when asked for, its gradient).
+    want_curves={name: end} (fixed design only, up to 1024 rows; names "lmp", "wind_mw", "batt_mw"): the exact NPV from the input
+    value of each parameter up to end (+inf allowed; "lmp" walks every hour on its own) in PriceTakerResult.curves, at most max_events
+    events per walk; the returned schedule is the vertex (one crossover serves the ranges too)."""
     T = int(n_time_points)
     design = bool(input_params.get("design_opt", False))
+    if want_curves and design:
+        raise NotImplementedError("want_curves needs a fixed design (design_opt=False)")
     if want_sensitivities and design:
         raise NotImplementedError("want_sensitivities needs a fixed design (design_opt=False)")
     if want_ranges and design:
@@ -221,14 +325,18 @@ def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solut
         rp = rp[0]
     elif rp.shape[0] != lmp.shape[0]:
         raise ValueError("sizes / capacity factors must be scalar or match the number of LMP scenarios")
-    marginal = ranges = None
-    if want_sensitivities or want_ranges:
-        dirs = _wind_directions(T, cf, lmp.shape[0]) if want_ranges else None
-        r, dc, dr, lo, hi = _solve_on_device(sol, lmp, rp, want_sensitivities, dirs)
+    marginal = ranges = curves = None
+    if want_sensitivities or want_ranges or want_curves:
+        N = lmp.shape[0]
+        dirs = _wind_directions(T, cf, N) if want_ranges else None
+        walks = _wind_walks(T, cf, N, lmp, input_params, want_curves) if want_curves else None
+        r, dc, dr, lo, hi, c = _solve_on_device(sol, lmp, rp, want_sensitivities, dirs, walks and walks[:3], max_events)
         if want_sensitivities:
-            marginal = _wind_marginals(T, cf, dc, dr, lmp.shape[0])
+            marginal = _wind_marginals(T, cf, dc, dr, N)
         if want_ranges:
             ranges = _wind_ranges(T, lmp, input_params, lo, hi)
+        if want_curves:
+            curves = _wind_curves(c, walks)
     else:
         r = sol.solve_host(lmp, rp, want_x=want_solution)
     if verbose:
@@ -240,7 +348,8 @@ def wind_battery_optimize(n_time_points, input_params, verbose=False, want_solut
     xm = sol.to_model_space(r.x) if want_solution else None
     if design:                                        # optimised size: value(m.battery_system_capacity)
         sizes["batt_kw"] = xm[:, sol.t.col_names.index("blk[0].fs.battery.nameplate_power")].copy()
-    return PriceTakerResult("wind_battery", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes, marginal, ranges=ranges)
+    return PriceTakerResult("wind_battery", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes, marginal, ranges=ranges,
+                            curves=curves)
 
 
 def _wind_battery_free_wind(T, lmp, cf, input_params, verbose):
@@ -278,12 +387,15 @@ def _wind_battery_free_wind(T, lmp, cf, input_params, verbose):
 
 
 def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_solution=True, kernel=None, want_sensitivities=False,
-                              want_ranges=False):
+                              want_ranges=False, want_curves=None, max_events=256):
     """kernel: a solver.KERNEL_* choice (None: the library's default).  want_sensitivities (fixed design only): fill
     PriceTakerResult.marginal_npv (wind_mw, batt_mw, pem_mw, h2_price_per_kg, lmp).  want_ranges (fixed design only, templates of
     up to 1024 rows): solve, cross over to a vertex and fill PriceTakerResult.ranges (lmp, wind_mw, batt_mw, pem_mw,
-    h2_price_per_kg); the returned schedule is the vertex (and marginal_npv, when asked for, its gradient)."""
+    h2_price_per_kg); the returned schedule is the vertex (and marginal_npv, when asked for, its gradient).  want_curves={name: end}
+    (fixed design only; names "lmp", "wind_mw", "batt_mw", "pem_mw", "h2_price_per_kg"): as wind_battery_optimize's."""
     mode = input_params.get("design_opt", False)
+    if want_curves and mode is not False:
+        raise NotImplementedError("want_curves needs a fixed design (design_opt=False)")
     if want_sensitivities and mode is not False:
         raise NotImplementedError("want_sensitivities needs a fixed design (design_opt=False)")
     if want_ranges and mode is not False:
@@ -298,7 +410,7 @@ def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_sol
     batt = np.zeros(1) if pem_design else np.asarray(input_params["batt_mw"], float)   # "PEM" fixes the battery at 0 (:228)
     # without a battery the template drops its columns; the sensitivities and ranges keep them (bounded by a zero size through Umap),
     # so that d NPV / d batt_mw at 0 is the value of the first MW of battery, not only its cost, and batt_mw has a range
-    with_batt = bool(np.any(batt > 0)) or want_sensitivities or want_ranges
+    with_batt = bool(np.any(batt > 0)) or want_sensitivities or want_ranges or bool(want_curves)
     want_solution = want_solution or pem_design
     sol = get_solver("wind_battery_pem", T, kernel=kernel, with_battery=with_batt, extant_wind=bool(input_params.get("extant_wind", True)),
                      pem_design=pem_design)
@@ -309,14 +421,17 @@ def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_sol
         raise ValueError("sizes / capacity factors must be scalar or match the number of LMP scenarios")
     h2 = np.broadcast_to(np.asarray(input_params["h2_price_per_kg"], float), (N,))
     cp = np.ascontiguousarray(np.concatenate([lmp, h2[:, None]], axis=1))
-    marginal = ranges = None
-    if want_sensitivities or want_ranges:
+    marginal = ranges = curves = None
+    if want_sensitivities or want_ranges or want_curves:
         dirs = _wind_directions(T, cf, N, pem=True) if want_ranges else None
-        r, dc, dr, lo, hi = _solve_on_device(sol, cp, rp, want_sensitivities, dirs)
+        walks = _wind_walks(T, cf, N, lmp, dict(input_params, batt_mw=batt), want_curves, h2=h2) if want_curves else None
+        r, dc, dr, lo, hi, c = _solve_on_device(sol, cp, rp, want_sensitivities, dirs, walks and walks[:3], max_events)
         if want_sensitivities:
             marginal = _wind_marginals(T, cf, dc, dr, N, pem=True)
         if want_ranges:
             ranges = _wind_ranges(T, lmp, dict(input_params, batt_mw=batt), lo, hi, h2=h2)
+        if want_curves:
+            curves = _wind_curves(c, walks)
     else:
         r = sol.solve_host(cp, rp, want_x=want_solution)
     sizes = dict(wind_kw=np.broadcast_to(np.asarray(input_params["wind_mw"], float) * 1e3, (N,)),
@@ -325,32 +440,43 @@ def wind_battery_pem_optimize(time_points, input_params, verbose=False, want_sol
     xm = sol.to_model_space(r.x) if want_solution else None
     if pem_design:                                    # optimised size: value(m.pem_system_capacity)
         sizes["pem_kw"] = xm[:, sol.t.col_names.index("pem_system_capacity[0]")].copy()
-    return PriceTakerResult("wind_battery_pem", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes, marginal, ranges=ranges)
+    return PriceTakerResult("wind_battery_pem", T, lmp, r.obj, r.status, r.iters, xm, sol.t.col_names, sizes, marginal, ranges=ranges,
+                            curves=curves)
 
 
 def nuclear_dispatch_optimize(n_time_points, lmps, want_solution=False, kernel=None, want_sensitivities=False, want_ranges=False,
-                              **flowsheet_options):
+                              want_curves=None, max_events=256, **flowsheet_options):
     """kernel: a solver.KERNEL_* choice (None: the library's default).  want_sensitivities: fill PriceTakerResult.marginal_obj["lmp"]
     = d obj / d lmp [N,T] (the sizes are template constants, not parameters).  want_ranges (templates of up to 1024 rows): solve,
     cross over to a vertex and fill PriceTakerResult.ranges["lmp"]; the returned schedule is the vertex (and marginal_obj, when asked
-    for, its gradient)."""
+    for, its gradient).  want_curves={"lmp": end}: each hour's exact objective from its LMP up to end in PriceTakerResult.curves
+    (Curve.npv holds the objective here)."""
     T = int(n_time_points)
     lmp = np.ascontiguousarray(np.atleast_2d(np.asarray(lmps, float))[:, :T])
+    if want_curves and set(want_curves) - {"lmp"}:
+        raise ValueError(f"want_curves: unknown names {sorted(set(want_curves) - {'lmp'})} (known: ['lmp'])")
     sol = get_solver("nuclear", T, kernel=kernel, **flowsheet_options)
-    marginal = ranges = None
-    if want_sensitivities or want_ranges:
+    marginal = ranges = curves = None
+    if want_sensitivities or want_ranges or want_curves:
         N, Pc = lmp.shape[0], sol.t.Pc
-        dirs = (np.broadcast_to(np.eye(T, Pc), (N, T, Pc)), None) if want_ranges else None
-        r, dc, _, lo, hi = _solve_on_device(sol, lmp, None, want_sensitivities, dirs)
+        eye = np.broadcast_to(np.eye(T, Pc), (N, T, Pc))
+        dirs = (eye, None) if want_ranges else None
+        walks = None
+        if want_curves:
+            te, end = _walk_ends("lmp", lmp, want_curves["lmp"], N)
+            walks = (eye, None, te)
+        r, dc, _, lo, hi, c = _solve_on_device(sol, lmp, None, want_sensitivities, dirs, walks, max_events)
         if want_sensitivities:
             marginal = dict(lmp=dc[:, :T])
         if want_ranges:
             ranges = dict(lmp=_absolute(lmp, lo, hi))
+        if want_curves:
+            curves = dict(lmp=_curve(c, list(range(T)), lmp, end, 1.0))
     else:
         r = sol.solve_host(lmp, None, want_x=want_solution)
     return PriceTakerResult("nuclear", T, lmp, r.obj, r.status, r.iters,
                             sol.to_model_space(r.x) if want_solution else None, sol.t.col_names, {}, marginal_obj=marginal,
-                            ranges=ranges)
+                            ranges=ranges, curves=curves)
 
 
 _SOLAR_COST_KEYS = ("pv_cap_cost", "pv_op_cost", "batt_cap_cost_kw", "batt_cap_cost_kwh", "pem_cap_cost", "pem_op_cost", "pem_var_cost",

@@ -22,13 +22,13 @@ import os
 _LIB_PATH = Path(os.environ.get("DSP_LP_LIB", Path(__file__).resolve().parent / "csrc" / "libdsp_lp.so"))
 _lib = None
 
-OPTIMAL, MAX_ITER, NUMERICAL, INFEASIBLE = 0, 1, 2, 3
-STATUS_NAMES = {OPTIMAL: "optimal", MAX_ITER: "maxIterations", NUMERICAL: "error", INFEASIBLE: "infeasible"}
+OPTIMAL, MAX_ITER, NUMERICAL, INFEASIBLE, UNBOUNDED = 0, 1, 2, 3, 4
+STATUS_NAMES = {OPTIMAL: "optimal", MAX_ITER: "maxIterations", NUMERICAL: "error", INFEASIBLE: "infeasible", UNBOUNDED: "unbounded"}
 
 KERNEL_AUTO, KERNEL_BAND, KERNEL_STAGE, KERNEL_STAGE_V1, KERNEL_DENSE, KERNEL_DENSE_CLUSTER, KERNEL_BAND_SPLIT = 0, 1, 2, 3, 4, 5, 6
 
 EXPORTS = ["dsp_lp_template_create", "dsp_lp_template_set_matrix_params", "dsp_lp_template_set_stage_chain1", "dsp_lp_template_create_csr", "dsp_lp_template_create_dense", "dsp_lp_template_create_dense_with_matrix_params", "dsp_lp_template_create_dense_cluster", "dsp_lp_analyze_csr", "dsp_lp_template_info", "dsp_lp_template_destroy", "dsp_lp_template_set_stage_wb", "dsp_lp_default_opts", "dsp_lp_solve_batch",
-           "dsp_lp_solve_batch_host", "dsp_lp_sensitivities", "dsp_lp_crossover", "dsp_lp_ranging", "dsp_lp_launch_count", "dsp_lp_last_launch", "dsp_lp_last_error",
+           "dsp_lp_solve_batch_host", "dsp_lp_sensitivities", "dsp_lp_crossover", "dsp_lp_ranging", "dsp_lp_parametric", "dsp_lp_launch_count", "dsp_lp_last_launch", "dsp_lp_last_error",
            "dsp_lp_version", "dsp_lp_fp64_peak_tflops"]
 
 
@@ -120,6 +120,9 @@ def load_library():
     lib.dsp_lp_ranging.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 3 + [C.c_int32] + \
         [C.c_void_p] * 2 + [C.c_int64] + [C.c_void_p] * 6
     lib.dsp_lp_ranging.restype = C.c_int
+    lib.dsp_lp_parametric.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 3 + [C.c_int32] + \
+        [C.c_void_p] * 2 + [C.c_int64, C.c_void_p, C.c_int32] + [C.c_void_p] * 10
+    lib.dsp_lp_parametric.restype = C.c_int
     lib.dsp_lp_launch_count.restype = C.c_int64
     lib.dsp_lp_last_launch.argtypes = [C.POINTER(C.c_int32)] * 4
     lib.dsp_lp_last_launch.restype = C.c_int
@@ -183,6 +186,45 @@ class Ranges:
     dobj: object         # [N,K] obj(theta) = obj + dobj theta + d2obj theta^2 / 2 inside the range
     d2obj: object        # [N,K]
     status: object       # [N] OPTIMAL / NUMERICAL, or the basis' status where that was not OPTIMAL
+
+
+@dataclasses.dataclass
+class Curves:
+    """dsp_lp_parametric (include/dsp_lp.h): along every direction k, the optimal value of every LP as an event log of basis changes;
+    between event e and the next, obj(theta) = obj[e] + dobj[e] (theta - theta[e]) + d2obj[e] (theta - theta[e])^2 / 2"""
+    theta: object        # [N,K,S] the events, nondecreasing from 0; NaN from count on
+    obj: object          # [N,K,S] c'x + k at each event
+    dobj: object         # [N,K,S] right derivatives of the segment each event opens (NaN on the last event of an INFEASIBLE /
+    d2obj: object        # [N,K,S]  UNBOUNDED walk, which marks where the curve stops)
+    enter: object        # [N,K,S] int32 entering variable (n + i: artificial of row i; -1: a bound flip, or none)
+    leave: object        # [N,K,S] int32 leaving or flipped variable (-1: none)
+    leave_to: object     # [N,K,S] int8 the bound it goes to (0 / 2; -1: none)
+    count: object        # [N,K] events recorded
+    status: object       # [N,K] OPTIMAL / INFEASIBLE / UNBOUNDED / MAX_ITER / NUMERICAL, or the basis' status where that was not OPTIMAL
+    theta_end: object = None   # [N,K] where each walk was asked to stop (None: +inf)
+
+    def value(self, p):
+        """the curves at theta values p ([N,K,P], or broadcastable to it).  NaN below 0, past theta_end, where the walk has no events,
+        and past the last event of a walk that did not end OPTIMAL (INFEASIBLE / UNBOUNDED: the curve stops there; MAX_ITER /
+        NUMERICAL: it is not known past there)"""
+        import torch
+        th = self.theta
+        p = torch.as_tensor(p, dtype=th.dtype, device=th.device)
+        p = p.expand(th.shape[:2] + p.shape[2:]) if p.dim() == 3 else p.reshape(1, 1, -1).expand(th.shape[:2] + (p.numel(),))
+        stops = (self.status == INFEASIBLE) | (self.status == UNBOUNDED)
+        last = self.count - stops.to(self.count.dtype)                      # events that open a segment
+        valid = torch.arange(th.shape[2], device=th.device)[None, None, :] < last[..., None]
+        key = torch.where(valid, th, torch.full_like(th, float("inf")))
+        e = (torch.searchsorted(key.contiguous(), p.contiguous(), right=True) - 1).clamp(min=0)
+        g = lambda a: torch.gather(a, 2, e)
+        d = p - g(th)
+        out = g(self.obj) + g(self.dobj) * d + 0.5 * g(self.d2obj) * d * d
+        end = torch.gather(th, 2, (self.count - 1).clamp(min=0).long()[..., None])
+        short = self.status != OPTIMAL
+        bad = (last[..., None] < 1) | (p < 0) | (short[..., None] & (p > end))
+        if self.theta_end is not None:
+            bad = bad | (p > torch.as_tensor(self.theta_end, dtype=th.dtype, device=th.device).expand(th.shape[:2])[..., None])
+        return torch.where(bad, torch.full_like(out, float("nan")), out)
 
 
 def _i32(a):
@@ -438,6 +480,65 @@ class BatchLPSolver:
                                      vertex.row_basic.data_ptr(), int(K), ptr(dir_c), ptr(dir_r), int(per_lp), ptr(out.theta_lo),
                                      ptr(out.theta_hi), ptr(out.dobj), ptr(out.d2obj), ptr(out.status), C.c_void_p(stream))
         self._check(rc, "dsp_lp_ranging")
+        return out
+
+    def parametric(self, cparams, rparams, vertex, dir_c=None, dir_r=None, theta_end=float("inf"), max_events=256):
+        """The optimal value of every LP along every direction, walked from the bases of a ``crossover`` result (a Vertex, or any object
+        with status, col_status and row_basic CUDA tensors) for the same cparams / rparams, m <= 1024: theta from 0 to theta_end (a
+        scalar, [K], or [N,K] with per-LP directions; +inf allowed), at most max_events events per walk.  dir_c [K,Pc] / dir_r [K,Pr]
+        shared by the batch, or [N,K,Pc] / [N,K,Pr] one set per LP (either may be None: those parameters do not move).  One kernel
+        launch on torch's current stream; the call waits for the stream up to the point where theta_end is ready, to check it."""
+        import torch
+        t = self.t
+        if not torch.is_tensor(cparams) or not cparams.is_cuda or cparams.dtype != torch.float64 or cparams.dim() != 2 \
+                or cparams.shape[1] != t.Pc:
+            raise ValueError(f"cparams must be a CUDA float64 tensor of shape [N, {t.Pc}]")
+        N = cparams.shape[0]
+        dev = cparams.device
+        ok = lambda a, shape, dt: torch.is_tensor(a) and a.is_cuda and a.device == dev and a.is_contiguous() and tuple(a.shape) == shape \
+            and a.dtype == dt
+        if not (ok(vertex.status, (N,), torch.int32) and ok(vertex.col_status, (N, t.n), torch.int8)
+                and ok(vertex.row_basic, (N, t.m), torch.int8)):
+            raise ValueError(f"vertex.status / col_status / row_basic must be contiguous CUDA [{N}] int32, [{N}, {t.n}] and [{N}, {t.m}] "
+                             f"int8 tensors")
+        cparams = cparams.contiguous()
+        rstride, rptr = 0, None
+        if t.Pr:
+            if rparams is None or not torch.is_tensor(rparams) or not rparams.is_cuda or rparams.dtype != torch.float64 \
+                    or rparams.device != dev or tuple(rparams.shape) not in ((t.Pr,), (N, t.Pr)):
+                raise ValueError(f"rparams must be a CUDA float64 tensor of shape [{t.Pr}] or [{N}, {t.Pr}] on {dev}")
+            rparams = rparams.contiguous()
+            rstride = 0 if rparams.dim() == 1 else t.Pr
+            rptr = rparams.data_ptr()
+        dirs = [d for d in (dir_c, dir_r) if d is not None]
+        if not dirs or not all(torch.is_tensor(d) and d.dim() in (2, 3) for d in dirs):
+            raise ValueError("dir_c / dir_r: at least one CUDA float64 tensor of shape [K, P] or [N, K, P]")
+        per_lp = dirs[0].dim() == 3
+        K = dirs[0].shape[-2]
+        for d, P, what in ((dir_c, t.Pc, "dir_c"), (dir_r, t.Pr, "dir_r")):
+            want = (N, K, P) if per_lp else (K, P)
+            if d is not None and (not torch.is_tensor(d) or not d.is_cuda or d.device != dev or d.dtype != torch.float64
+                                  or tuple(d.shape) != want):
+                raise ValueError(f"{what} must be a CUDA float64 tensor of shape {list(want)} on {dev}")
+        dir_c = dir_c.contiguous() if dir_c is not None else None
+        dir_r = dir_r.contiguous() if dir_r is not None else None
+        te_shape = (N, K) if per_lp else (K,)
+        te = torch.as_tensor(theta_end, dtype=torch.float64, device=dev)
+        if te.dim() > len(te_shape) or tuple(te.shape) not in (te_shape, (), te_shape[-1:]):
+            raise ValueError(f"theta_end must be a scalar or of shape {list(te_shape)}")
+        te = te.expand(te_shape).contiguous()
+        S_ = int(max_events)
+        e = lambda shape, dt: torch.empty(shape, dtype=dt, device=dev)
+        out = Curves(e((N, K, S_), torch.float64), e((N, K, S_), torch.float64), e((N, K, S_), torch.float64), e((N, K, S_), torch.float64),
+                     e((N, K, S_), torch.int32), e((N, K, S_), torch.int32), e((N, K, S_), torch.int8), e((N, K), torch.int32),
+                     e((N, K), torch.int32), te.expand(N, K) if not per_lp else te)
+        ptr = lambda a: a.data_ptr() if a is not None and a.numel() else None
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        rc = self.lib.dsp_lp_parametric(self.handle, N, ptr(cparams), rptr, rstride, vertex.status.data_ptr(), vertex.col_status.data_ptr(),
+                                        vertex.row_basic.data_ptr(), int(K), ptr(dir_c), ptr(dir_r), int(per_lp), ptr(te), S_,
+                                        ptr(out.theta), ptr(out.obj), ptr(out.dobj), ptr(out.d2obj), ptr(out.enter), ptr(out.leave),
+                                        ptr(out.leave_to), ptr(out.count), ptr(out.status), C.c_void_p(stream))
+        self._check(rc, "dsp_lp_parametric")
         return out
 
     def crossover(self, cparams, rparams, result, max_pivots=0):

@@ -141,6 +141,7 @@ int dsp_lp_template_set_stage_chain1(dsp_template *t, const dsp_stage_chain1_des
  * iters counts the iterations of both attempts: an LP whose first attempt ends non-optimal is solved again (shorter step, stronger
  * proximal term) and reports first + second, so with max_iter = k a non-optimal LP reports 2k.                              */
 enum { DSP_OPTIMAL = 0, DSP_MAX_ITER = 1, DSP_NUMERICAL = 2, DSP_INFEASIBLE = 3 };
+enum { DSP_UNBOUNDED = 4 };        /* only dsp_lp_parametric returns it: the LP is unbounded past a breakpoint */
 enum { DSP_E_ARG = -1, DSP_E_CUDA = -2, DSP_E_SMEM = -3, DSP_E_BUSY = -4 /* a host call is already in flight on this handle */ };
 
 /* Replaces: the per-LP model hand-over inside SolverFactory(..).solve(m) (Pyomo LP/NL writer), done once. */
@@ -308,6 +309,60 @@ int dsp_lp_ranging(const dsp_template *t, int64_t N,
                    double *theta_lo /*[N,K]*/, double *theta_hi /*[N,K]*/,
                    double *dobj /*[N,K] or NULL*/, double *d2obj /*[N,K] or NULL*/,
                    int32_t *rstatus /*[N]*/, void *cuda_stream);
+
+/* Parametric walk over given bases: for every LP and every direction k, the exact optimal value of the LP at the parameters
+ * (cp + theta dir_c[k], rp + theta dir_r[k]) for theta from 0 up to theta_end[k] (+inf allowed), as an event log of the basis changes
+ * along the way; a parametric simplex from dsp_lp_ranging's range to the next basis, repeated.  m <= 1024.
+ * The LP and the basis are dsp_lp_ranging's (col_status [N,n], row_basic [N,m], xstatus [N], e.g. dsp_lp_crossover's outputs); the basis
+ * must be optimal at theta = 0.  At every theta the LP is formed afresh from the parameters, p + theta dir with one fma each.
+ * Outputs per (LP, direction) pair, [N,K,S] (S events at most) and [N,K]:
+ *   event 0: theta = 0, obj = c'x + k of the basis, enter = leave = leave_to = -1;
+ *   event e >= 1: one basis change or bound flip at theta[e] >= theta[e-1]; obj[e] recomputed from the new basis there; enter the
+ *     entering variable (n + i: the artificial of row i; -1 for a bound flip), leave the leaving or flipped variable, leave_to the
+ *     bound it goes to (0: at 0, 2: at u);
+ *   dobj[e], d2obj[e]: the right derivatives of the segment that starts at event e, so that up to the next event (or theta_end)
+ *     obj(theta) = obj[e] + dobj[e] (theta - theta[e]) + d2obj[e] (theta - theta[e])^2 / 2 exactly (d2obj = 0 unless the direction
+ *     moves both c and b / u).  Events at equal theta are degenerate pivots; the last of them defines the segment.  Applying the
+ *     events in order to the start basis gives the basis of every segment.  The curve is convex along a direction that moves only b / u
+ *     and concave along one that moves only c;
+ *   a walk that ends INFEASIBLE or UNBOUNDED has a last event at the breakpoint with enter = leave = leave_to = -1 and NaN dobj / d2obj:
+ *     the curve stops there;
+ *   entries from count on are NaN (-1 for enter / leave / leave_to).
+ * pstatus [N,K]: DSP_OPTIMAL (the walk reached theta_end, or no basis change happens past the last event), DSP_INFEASIBLE (past the
+ * last event no point is feasible: a dual simplex step finds no entering column, or an upper bound at which a column sits reaches 0),
+ * DSP_UNBOUNDED (past the last event the objective is unbounded below), DSP_MAX_ITER (S events before theta_end; the log so far is
+ * kept), DSP_NUMERICAL (the start basis is not a basis with every nonbasic column at a finite bound, its reinversion is singular, it is
+ * not primal and dual feasible within dsp_lp_ranging's tolerances, or after an event a reinversion is singular or the basis is primal
+ * and dual infeasible at once; a direction with a nonzero dir_r entry on a parameter that enters a matrix term, which moves A, gets
+ * count 0 and NaN rows), or the input xstatus where that is not DSP_OPTIMAL (count 0, NaN rows).
+ * Rules at a breakpoint (csrc/dsp_parametric.cuh, DESIGN.md 4.8): the blocking entry of the range is the one with the smallest ratio,
+ * primal before dual, then the lowest variable index; a basic variable at a bound leaves by a dual simplex pivot, a reduced cost at 0
+ * enters by a primal simplex pivot (or flips to its other bound), each ratio test ordered by (ratio, its derivative in theta, the
+ * larger |alpha|, index) so that the new basis stays optimal just past the breakpoint; a fixed column (u = 0) that the direction
+ * unfixes at the bound its reduced cost does not ask for flips at once.  After 50 zero-length events in a row, ratio-test ties go to
+ * the lowest index (not Bland's rule: a walk that cycles ends DSP_MAX_ITER at S events).  An artificial leaves to 0 (leave_to 0).
+ * Exactness: on every template the tests cover, each segment's objective is the exact optimum to 1e-9 relative and each breakpoint
+ * the exact end of its basis' range to 1e-8.  On LPs with redundant rows and long degenerate stretches (the PV + battery + hydrogen
+ * design templates) a replayed segment basis may miss exact optimality by a rounding-sized violation (a degenerate basic variable at
+ * about -1e-13 after a primal pivot whose ratio test skips it: its entry in the pivot column is below the pivot tolerance); the
+ * objective and breakpoints still hold to those bars.
+ * Directions: dir_c / dir_r as dsp_lp_ranging's (shared with dir_stride == 0, else per LP); theta_end [K], or [N,K] per LP.  One CTA
+ * per (LP, direction) pair.  DEVICE pointers, stream-ordered; the call reads theta_end back to check it (it waits for the stream up
+ * to that point), the walks run asynchronously.  The rparams_stride == 0 broadcast of dsp_lp_solve_batch.  Results are bitwise
+ * reproducible and do not depend on where a pair sits in the batch.  One kernel launch per call (none when N == 0 or K == 0).
+ * DSP_E_ARG: NULL handle, N < 0, K < 0, S < 1, m > 1024 ("parametric takes m <= 1024"), and for N > 0 and K > 0 NULL xstatus /
+ * col_status / row_basic / theta / obj / dobj / count / pstatus, NULL theta_end or a negative or NaN entry of it, NULL cparams with
+ * Pc > 0 or NULL rparams with Pr > 0. */
+int dsp_lp_parametric(const dsp_template *t, int64_t N,
+                      const double *cparams, const double *rparams, int64_t rparams_stride,
+                      const int32_t *xstatus, const int8_t *col_status, const int8_t *row_basic,
+                      int32_t K, const double *dir_c /*[K,Pc] or NULL*/, const double *dir_r /*[K,Pr] or NULL*/,
+                      int64_t dir_stride /* 0: shared by the batch; else per LP, [N,K,Pc] / [N,K,Pr] */,
+                      const double *theta_end /*[K], or [N,K] when dir_stride != 0; each >= 0, +inf allowed*/,
+                      int32_t S /* events per walk, >= 1 */,
+                      double *theta /*[N,K,S]*/, double *obj /*[N,K,S]*/, double *dobj /*[N,K,S]*/, double *d2obj /*[N,K,S] or NULL*/,
+                      int32_t *enter /*[N,K,S] or NULL*/, int32_t *leave /*[N,K,S] or NULL*/, int8_t *leave_to /*[N,K,S] or NULL*/,
+                      int32_t *count /*[N,K]*/, int32_t *pstatus /*[N,K]*/, void *cuda_stream);
 
 /* Introspection used by tests / bench: kernel launches issued so far, last launch geometry (grid in CTAs, block, dynamic shared
  * memory; problems_per_cta: LPs per CTA, or for the dense cluster kernel the cluster size in CTAs). */
